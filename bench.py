@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- aligned Gbp/s of the convex-gap banded alignment hot path on B200.
+"""bench.py -- aligned Gbp/s of the convex-gap banded alignment hot path on H100.
 
 One "step" = one pass of the hot path over one batch of synthetic PacBio-shaped reads: stage 0/2
 (k-mer candidate search of every 256-bp sub-read, device-side window decode and StrippedSW scoring
@@ -19,6 +19,9 @@ one NCCL broadcast of the reference at start-up).
 
 `--impl reference` times the CPU implementation instead (all host threads) and prints the same
 line with "impl": "reference".
+
+`--dump-outputs DIR` writes what the device-resident timed path computed in its last step (rank 0) as
+DIR/<name>.npy; the inputs are seeded, so two builds can be compared output for output.
 """
 import argparse
 import json
@@ -85,7 +88,7 @@ class Workload:
 
 
 class ClockSampler:
-    """nvidia-smi clocks/throttle reasons DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks/throttle reasons DURING the timed region."""
     Q = ("timestamp,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,"
          "clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -143,6 +146,17 @@ class ClockSampler:
                     reasons.add(name)
         return {"sm_mhz": float(np.median(sm)) if sm else None, "sm_max_mhz": max(mx) if mx else None,
                 "reasons": sorted(reasons), "samples": len(sm)}
+
+
+def gpu_identity(gpu_index):
+    """Card name and power limit: part of every absolute number this benchmark prints."""
+    try:
+        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader,nounits",
+                              "-i", str(gpu_index)], capture_output=True, text=True, timeout=30).stdout.strip()
+        name, watts = [x.strip() for x in out.split(",")[:2]]
+        return {"name": name, "power_limit_w": float(watts)}
+    except Exception:
+        return {"name": None, "power_limit_w": None}
 
 
 class CpuStage02:
@@ -558,6 +572,58 @@ def integrated_run(wl_cfg, genome, contig_len, n_contigs, enc_ref, index, n_read
         shutil.rmtree(d, ignore_errors=True)
 
 
+DUMP_CANDIDATES = 1 << 20   # candidates written in full up to this many, else a seeded sample of this size
+
+
+def dump_outputs(out_dir, als, with_stage02):
+    """What the device-resident timed path computed in its last step, as its caller receives it: every context's
+    alignments (fetch) and, with stage 0/2, its candidates and their scores (cs_fetch), contexts in order. CIGAR
+    and MD text enter as their CRC-32 and length. At most 64 MB in all: beyond DUMP_CANDIDATES candidates a fixed,
+    seeded sample of them is written (cand_index = their positions in the concatenated list)."""
+    import zlib
+    os.makedirs(out_dir, exist_ok=True)
+    out = {}
+    ints = ("ret", "position_offset", "qstart", "qend", "nm", "alignment_length", "cigar_op_count", "sv_type")
+    cols = {k: [] for k in ints + ("score", "identity", "cigar_crc32", "cigar_len", "md_crc32", "md_len")}
+    for a in als:
+        res = a.fetch()
+        for i in range(len(res)):
+            d = res[i].as_dict()
+            for k in ints:
+                cols[k].append(d[k])
+            cols["score"].append(d["score"])
+            cols["identity"].append(res[i].Identity)
+            for k, s in (("cigar", d["cigar"]), ("md", d["md"])):
+                b = s.encode() if isinstance(s, str) else bytes(s)
+                cols[k + "_crc32"].append(zlib.crc32(b))
+                cols[k + "_len"].append(len(b))
+    for k, v in cols.items():
+        out["aln_" + k] = np.asarray(v, dtype=np.float32 if k in ("score", "identity") else np.float64)
+    if with_stage02:
+        starts, parts, base = [], {k: [] for k in ("vote_score", "location", "reverse", "sw_score")}, 0
+        max_vote = []
+        for a in als:
+            cstart, sc, lo, rv, sw, mx = a.cs_fetch()
+            starts.append(cstart[:-1] + base)
+            base += int(cstart[-1])
+            for k, v in zip(parts, (sc, lo, rv, sw)):
+                parts[k].append(v)
+            max_vote.append(mx)
+        out["cand_start"] = np.concatenate(starts + [np.array([base])]).astype(np.float64)
+        out["cand_max_vote"] = np.concatenate(max_vote).astype(np.float32)
+        idx = np.arange(base)
+        if base > DUMP_CANDIDATES:
+            idx = np.sort(np.random.default_rng(0).choice(base, DUMP_CANDIDATES, replace=False))
+        out["cand_index"] = idx.astype(np.float64)
+        for k, v in parts.items():
+            out["cand_" + k] = np.concatenate(v)[idx].astype(np.float64 if k == "location" else np.float32)
+    total = sum(v.nbytes for v in out.values())
+    assert total <= 64 << 20, f"--dump-outputs: {total} bytes exceed 64 MB"
+    for k, v in out.items():
+        np.save(os.path.join(out_dir, k + ".npy"), v)
+    return total
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -585,6 +651,9 @@ def main():
     ap.add_argument("--integrated-reads", type=int, default=-1,
                     help="reads of the whole-ngmlr comparison (plain binary vs plugin-linked binary); "
                          "-1 = 2000 at N=1 on configs up to 100 Mb, else 0 (skipped)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps write what the device-resident path computed in its last step "
+                         "(rank 0) as DIR/<name>.npy")
     args = ap.parse_args()
     if args.warmup < 3 and args.impl == "b200":
         args.warmup = 3
@@ -641,7 +710,7 @@ def main():
         print(json.dumps(line))
         return
 
-    # ------------------------------------------------------------------ B200 arm
+    # ------------------------------------------------------------------ GPU arm
     import torch
     import torch.distributed as dist
 
@@ -782,6 +851,8 @@ def main():
     sampler.mark_end()
     clocks = sampler.stop()
     dev_ms = e0.elapsed_time(e1)
+    if args.dump_outputs and rank == 0:   # before the end-to-end phase reuses the contexts
+        dump_outputs(args.dump_outputs, als, not args.dp_only)
 
     # ---- (c) end to end from host buffers through the public calls: per step every context uploads its
     # reads ONCE (reads_upload), runs stage 0/2 on their sub-reads and brings candidates + scores back
@@ -838,33 +909,18 @@ def main():
             peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         except Exception:
             pass
-        peak = float(peaks.get("hbm_gbs", 6650.0))
-        peak_src = "measured (MEASURED_PEAKS.json hbm_gbs, burst)" if peaks else "fallback 6650 GB/s"
+        peak = float(peaks.get("hbm_gbs", 3350.0))
+        peak_src = "measured (MEASURED_PEAKS.json hbm_gbs, burst)" if peaks else "H100 SXM data sheet 3350 GB/s"
         # algorithmic bytes of ONE fill launch (DESIGN.md section 4): 0.25 B per DP cell (2-bit direction) +
         # sequences read once; corridor rows are generated on the device from 28-byte closed forms
         seq_b = sum(iv.ref_len + iv.read_len for iv in wl.ivs)
         algo_bytes = cells * 0.25 + seq_b + 112 * len(wl.ivs)
         fill_s = float(np.mean(fill_ms)) * 1e-3
         achieved = algo_bytes / fill_s / 1e9
-        sm_mhz = float(clocks.get("sm_mhz") or 1965.0)
-        # SURVEY section 8(d): 148 SMs x 128 lanes x clock / >= 25 instructions per cell
-        issue_bound = 148 * 128 * sm_mhz * 1e6 / 25.0
-        traffic = None
-        alu_ops = lane_instr = None
-        try:  # DRAM bytes of one fill launch from the committed ncu capture (same workload only)
-            tr = json.load(open(os.path.join(ROOT, "profiles", "fill_traffic.json")))
-            if tr.get("reads_per_step") == args.reads and tr.get("config", "pacbio50") == args.config:
-                traffic = tr["dram_bytes_per_launch"]
-            alu_ops = tr.get("alu_pipe_lane_ops_per_cell")   # a property of the kernel's code, not of the batch
-            lane_instr = tr.get("lane_instructions_per_cell")
-        except Exception:
-            pass
-        # the pipe that binds (DESIGN.md 4.1): compares / selects / min-max run on the ALU pipe only, 16 lanes per
-        # clock and SM sub-partition; ops per cell from the same ncu capture
-        alu_bound = 148 * 4 * 16 * sm_mhz * 1e6 / alu_ops if alu_ops else None
-        # what the kernel's own instruction count allows at one warp-instruction per clock and sub-partition (the
-        # final build issues 67.4 lane-instructions per useful cell incl. block ramp and chunk hand-off)
-        own_issue_bound = 148 * 128 * sm_mhz * 1e6 / lane_instr if lane_instr else None
+        sm_mhz = float(clocks.get("sm_mhz") or clocks.get("sm_max_mhz") or 1980.0)
+        n_sms = torch.cuda.get_device_properties(dev).multi_processor_count
+        # SURVEY section 8(d): SMs x 128 lanes x clock / >= 25 instructions per cell
+        issue_bound = n_sms * 128 * sm_mhz * 1e6 / 25.0
         line = {
             "metric": "aligned_gbp_per_s", "value": value, "unit": "Gbp/s", "n_gpus": world,
             "steps": args.steps, "warmup": args.warmup, "ms_per_step": dev_ms / args.steps,
@@ -884,20 +940,14 @@ def main():
             "reads_per_s": args.reads * world * args.steps / (dev_ms * 1e-3),
             "gcells_per_s": tot_cells * args.steps / (dev_ms * 1e-3) / 1e9,
             "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s",
-                         "frac": achieved / peak, "traffic": traffic, "peak_source": peak_src,
+                         "frac": achieved / peak, "peak_source": peak_src,
                          "kernel": "convex_fill_kernel", "launch_ms": fill_s * 1e3,
                          "algorithmic_bytes_per_launch": algo_bytes,
                          "gcells_per_s_kernel": cells / fill_s / 1e9,
                          "issue_bound_gcells_per_s": issue_bound / 1e9,
                          "frac_of_issue_bound": cells / fill_s / issue_bound,
-                         "alu_pipe_bound_gcells_per_s": alu_bound / 1e9 if alu_bound else None,
-                         "frac_of_alu_pipe_bound": cells / fill_s / alu_bound if alu_bound else None,
-                         "own_instruction_count_bound_gcells_per_s": own_issue_bound / 1e9 if own_issue_bound else None,
-                         "frac_of_own_instruction_count_bound": cells / fill_s / own_issue_bound if own_issue_bound else None,
-                         "note": "integer/float DP: instruction-issue bound (SURVEY 8(d): 148 SMs x 128 lanes x clock / "
-                                 "25 instructions per cell), not HBM bound; the HBM fraction is structurally ~0.02. The "
-                                 "kernel issues 67.4 lane-instructions per useful cell (ncu, profiles/fill_traffic.json): "
-                                 "issue slots 85 % busy, ALU pipe 67 %"},
+                         "note": f"integer/float DP: instruction-issue bound (SURVEY 8(d): {n_sms} SMs x 128 lanes x "
+                                 "clock / 25 instructions per cell), not HBM bound"},
             "kernel_ms_per_step": {"fill": float(np.mean(fill_ms)), "traceback": float(np.mean(tb_ms)),
                                    "text": float(np.mean(tx_ms)),
                                    "stage02_cs_vote_decode_score": float(np.mean(cs_ms))},
@@ -919,6 +969,7 @@ def main():
             # per context and step: cs count, sizes, 4 x (scan init + scan), vote, count widening, compaction,
             # window decode + score (14) + fill, traceback, text (3)
             "gpu_launches": (3 if args.dp_only else 17) * S * args.steps,
+            "gpu": dict(gpu_identity(local_rank), sms=n_sms),
             "clocks": clocks,
         }
         # CPU baseline on this box's host cores, bounded sample of the same workload -- and the parity check:
@@ -948,7 +999,7 @@ def main():
                                     "sample": repr(ex)}
         try:   # the plugin surface itself, on the first context's slice of the batch
             k_ = len(wl.ivs) if len(wl.ivs) <= 2048 else 2048
-            line["e2e_ialignment"] = ialignment_batch_align(wl, wl.ivs[:k_], gpu_first[:k_], max(2, args.steps // 2),
+            line["e2e_ialignment"] = ialignment_batch_align(wl, wl.ivs[:k_], gpu_first[:k_], args.steps,
                                                             local_rank)
         except AssertionError:
             raise

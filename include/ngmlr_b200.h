@@ -1,4 +1,4 @@
-/* include/ngmlr_b200.h -- C ABI of the B200-native ngmlr alignment hot path.
+/* include/ngmlr_b200.h -- C ABI of the H100-native ngmlr alignment hot path.
  *
  * libngmlr_b200.so exports two surfaces:
  *

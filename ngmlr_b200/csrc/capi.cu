@@ -82,9 +82,15 @@ int ngmlr_b200_create(int gpu_id, const ngmlr_b200_scoring* s, ngmlr_b200_ctx** 
   cudaDeviceProp prop;
   cudaGetDeviceProperties(&prop, gpu_id);
   ctx->num_sms = prop.multiProcessorCount;
-  if (prop.major != 10 || prop.minor != 0) {  // only sm_100a SASS is embedded (no PTX for other architectures)
-    g_create_error = "ngmlr_b200: kernels are built for sm_100a only; device is sm_" +
+  if (prop.major != 9 || prop.minor != 0) {  // only sm_90a SASS is embedded (no PTX for other architectures)
+    g_create_error = "ngmlr_b200: kernels are built for sm_90a only; device is sm_" +
                      std::to_string(prop.major) + std::to_string(prop.minor);
+    delete ctx;
+    return -1;
+  }
+  ctx->sm_ids = fill_sm_id_bound();
+  if (ctx->sm_ids <= 0) {
+    g_create_error = "ngmlr_b200: could not read the SM id range of the device";
     delete ctx;
     return -1;
   }

@@ -1,4 +1,4 @@
-// ngmlr_b200/csrc/convex_fill.cu -- convex-gap banded Smith-Waterman forward fill for sm_100a.
+// ngmlr_b200/csrc/convex_fill.cu -- convex-gap banded Smith-Waterman forward fill for sm_90a.
 //
 // Replaces Convex::ConvexAlignFast::fwdFillMatrixSSESimple (src/ConvexAlignFast.cpp:914-1287)
 // over Convex::AlignmentMatrixFast (src/AlignmentMatrixFast.{h,cpp}).
@@ -611,6 +611,24 @@ int fill_max_ctas_per_sm(bool raw, bool team) {
     else cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, convex_fill_kernel<false, 1, true>, threads, 0);
   }
   return n;
+}
+
+namespace {
+__global__ void nsmid_kernel(unsigned* out) {
+  unsigned v;
+  asm("mov.u32 %0, %%nsmid;" : "=r"(v));
+  *out = v;
+}
+}  // namespace
+
+int fill_sm_id_bound() {
+  unsigned* d = nullptr;
+  unsigned h = 0;
+  if (cudaMalloc(&d, sizeof(unsigned)) != cudaSuccess) return -1;
+  nsmid_kernel<<<1, 1>>>(d);
+  const bool ok = cudaMemcpy(&h, d, sizeof(unsigned), cudaMemcpyDeviceToHost) == cudaSuccess;
+  cudaFree(d);
+  return ok ? (int)h : -1;
 }
 
 }  // namespace nb

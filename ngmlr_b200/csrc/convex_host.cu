@@ -433,12 +433,12 @@ int ngmlr_b200_convex_run(ngmlr_b200_ctx* ctx) {
   const bool persistent = ctx->fill_ctas_cap > 0 || ctx->fill_persistent;
   const int grid = persistent ? std::max(1, std::min(max_grid, want_grid)) : std::max(1, want_grid);
   ctx->fill_grid = grid;
-  const size_t strips = persistent ? (size_t)grid : (size_t)ctx->num_sms * FILL_SM_SLOTS;
+  const size_t strips = persistent ? (size_t)grid : (size_t)ctx->sm_ids * FILL_SM_SLOTS;
   const size_t warps = strips * (team ? 1 : FILL_WARPS_PER_CTA);  // a team shares one strip
   if (!persistent) {
-    CU(ctx->d_sm_slots.reserve((size_t)ctx->num_sms + 8));
+    CU(ctx->d_sm_slots.reserve((size_t)ctx->sm_ids));
     if (!ctx->sm_slots_zeroed) {
-      CU(cudaMemsetAsync(ctx->d_sm_slots.p, 0, ((size_t)ctx->num_sms + 8) * sizeof(unsigned int), st));
+      CU(cudaMemsetAsync(ctx->d_sm_slots.p, 0, (size_t)ctx->sm_ids * sizeof(unsigned int), st));
       ctx->sm_slots_zeroed = true;
     }
   }

@@ -1,4 +1,4 @@
-// ngmlr_b200/csrc/convex_text.cu -- CIGAR / MD / NM text and the inversion-peak scan on the device (sm_100a).
+// ngmlr_b200/csrc/convex_text.cu -- CIGAR / MD / NM text and the inversion-peak scan on the device (sm_90a).
 //
 // Replaces, for a whole batch, the text half of Convex::ConvexAlignFast::SingleAlign:
 //   convertCigar   (src/ConvexAlignFast.cpp:112-333, addPosition :76-99)  binary CIGAR -> CIGAR and

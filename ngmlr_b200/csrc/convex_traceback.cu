@@ -1,4 +1,4 @@
-// ngmlr_b200/csrc/convex_traceback.cu -- traceback + binary-CIGAR emission for sm_100a.
+// ngmlr_b200/csrc/convex_traceback.cu -- traceback + binary-CIGAR emission for sm_90a.
 //
 // Replaces Convex::ConvexAlignFast::revBacktrack (src/ConvexAlignFast.cpp:335-432) with
 // AlignmentMatrixFast::getDirection / validPath (src/AlignmentMatrixFast.cpp:185-195, 213-220).

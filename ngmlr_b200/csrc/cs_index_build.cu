@@ -1,4 +1,4 @@
-// ngmlr_b200/csrc/cs_index_build.cu -- construction of the k-mer index on the device (sm_100a).
+// ngmlr_b200/csrc/cs_index_build.cu -- construction of the k-mer index on the device (sm_90a).
 //
 // Replaces CompactPrefixTable::CreateTable for one table unit (src/PrefixTable.cpp:323-370):
 //   CountKmerFreq / CountKmer        (:199-231, :372-394)  k-mer frequencies of the reference
@@ -241,7 +241,7 @@ cudaError_t build_kmer_index(const IndexBuildParams& p, IndexBuildScratch& s, cu
     if (e__ != cudaSuccess) return e__; \
   } while (0)
   const int threads = 256;
-  const int grid = 148 * 16;
+  const int grid = current_device_sms() * 16;
   const uint32_t n_kmers = 1u << (2 * p.k);
   const long long cl = (long long)p.concat_len;  // 64-bit item counts: a human genome has > 2^31 bases
   // ---- 1. callbacks ----

@@ -1,4 +1,4 @@
-// ngmlr_b200/csrc/cs_search.cu -- k-mer candidate search (stage 0) for sm_100a.
+// ngmlr_b200/csrc/cs_search.cu -- k-mer candidate search (stage 0) for sm_90a.
 //
 // Replaces, per (sub-)read, CS::RunRead's search (src/CS.cpp:324-398): CS::PrefixIteration
 // (src/CSstatic.cpp:23-73) -> CS::PrefixSearch (src/CS.cpp:57-96) ->

@@ -1,4 +1,4 @@
-// ngmlr_b200/csrc/device_types.h -- records shared between host runtime and sm_100a kernels.
+// ngmlr_b200/csrc/device_types.h -- records shared between host runtime and sm_90a kernels.
 #pragma once
 #include <stdint.h>
 #include <vector_types.h>  // int4

@@ -1,4 +1,4 @@
-// ngmlr_b200/csrc/kernels.h -- launchers of the sm_100a kernels (host-callable).
+// ngmlr_b200/csrc/kernels.h -- launchers of the sm_90a kernels (host-callable).
 #pragma once
 #include <cuda_runtime.h>
 
@@ -25,6 +25,16 @@ cudaError_t launch_convex_fill(const FillParams& p, bool raw, bool team, int gri
 // the same kernel with a FILL_BIG_TEAM-warp team per problem, for the huge matrices of a batch
 cudaError_t launch_convex_fill_big(const FillParams& p, bool raw, int grid, cudaStream_t stream);
 int fill_max_ctas_per_sm(bool raw, bool team);
+// %nsmid of the current device: every %smid is below it (SM ids need not be dense in 0 .. SM count - 1); -1 on error
+int fill_sm_id_bound();
+
+// SMs of the current device (grid caps of the grid-stride kernels)
+inline int current_device_sms() {
+  int dev = 0, n = 0;
+  cudaGetDevice(&dev);
+  cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
+  return n > 0 ? n : 1;
+}
 
 cudaError_t launch_convex_traceback(const TraceParams& p, cudaStream_t stream);
 

@@ -1,4 +1,4 @@
-// ngmlr_b200/csrc/ref_decode.cu -- reference windows for alignment, decoded on the device (sm_100a).
+// ngmlr_b200/csrc/ref_decode.cu -- reference windows for alignment, decoded on the device (sm_90a).
 //
 // Replaces _SequenceProvider::DecodeRefSequenceExact(sequence, startPosition, sequenceLength, 0)
 // (src/SequenceProvider.cpp:493-565 with decode :475-490 and getChrStart :157-178) as called by
@@ -123,7 +123,7 @@ cudaError_t launch_gather_reads(const GatherParams& p, cudaStream_t stream) {
 cudaError_t launch_encode_contig(const uint8_t* text, unsigned long long len, uint8_t* out, cudaStream_t stream) {
   if (!len) return cudaSuccess;
   const unsigned long long n_bytes = (len + 1ull) >> 1;
-  const int grid = (int)std::min<unsigned long long>((n_bytes + 255ull) / 256ull, 148ull * 32ull);
+  const int grid = (int)std::min<unsigned long long>((n_bytes + 255ull) / 256ull, (unsigned long long)current_device_sms() * 32ull);
   encode_contig_kernel<<<grid, 256, 0, stream>>>(text, len, out);
   return cudaGetLastError();
 }

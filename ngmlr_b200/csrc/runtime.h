@@ -181,6 +181,7 @@ constexpr int TEXT_SLOTS = 6;  // pinned result arenas: one per attempt of a com
 struct ngmlr_b200_ctx {
   int device = 0;
   int num_sms = 0;
+  int sm_ids = 0;                   // %nsmid: size of the per-SM slot table of the short-lived fill CTAs
   cudaStream_t stream = nullptr;
   cudaStream_t stream2 = nullptr;   // the big-team fill launch runs beside the ordinary one
   cudaStream_t stream_fill = nullptr;  // lowest priority: the launch of short-lived fill CTAs

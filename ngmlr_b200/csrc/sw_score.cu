@@ -1,4 +1,4 @@
-// ngmlr_b200/csrc/sw_score.cu -- score-only local alignment of sub-read x candidate pairs (sm_100a).
+// ngmlr_b200/csrc/sw_score.cu -- score-only local alignment of sub-read x candidate pairs (sm_90a).
 //
 // Replaces StrippedSW::BatchScore / SingleScore (src/StrippedSW.cpp:118-202) and the part of the
 // vendored SSW library they reach: ssw_init -> qP_word, ssw_align(flag=0) -> sw_sse2_word

@@ -72,10 +72,13 @@ def test_no_cpu_fallback():
     assert lib.CreateAlignment(0) is None  # plugin factory fails loudly too
 
 
-@pytest.mark.skipif(not os.path.isdir("/root/reference/src"), reason="reference headers not present")
+# what the probe below prints when compiled against the reference's own src/IAlignment.h (x86-64, g++)
+REFERENCE_IALIGNMENT_LAYOUT = "120 16 12 88 8 24 40 84 116 108 8 72 11 12 \n"
+
+
 def test_compat_header_layout_equals_reference_header():
     """sizeof/offsetof of Align, CorridorLine, PositionNM, Interval and the vtable slot order of
-    IAlignment in include/ngmlr_b200_ialignment.h == src/IAlignment.h."""
+    IAlignment in include/ngmlr_b200_ialignment.h == src/IAlignment.h (recorded above)."""
     probe = r'''
 #include <stdio.h>
 #include <stddef.h>
@@ -103,13 +106,10 @@ int main() {
   return 0;
 }'''
     import tempfile
-    outs = []
     with tempfile.TemporaryDirectory() as d:
-        for hdr, inc in (('"IAlignment.h"', "/root/reference/src"),
-                         ('"ngmlr_b200_ialignment.h"', os.path.join(ROOT, "include"))):
-            path = os.path.join(d, "p.cpp")
-            open(path, "w").write(probe.replace("HEADER", hdr))
-            subprocess.run(["g++", "-std=c++11", "-w", "-I", inc, "-o", os.path.join(d, "p"), path,
-                            "-Wl,--unresolved-symbols=ignore-all"], check=True)
-            outs.append(subprocess.run([os.path.join(d, "p")], capture_output=True, text=True, check=True).stdout)
-    assert outs[0] == outs[1], outs
+        path = os.path.join(d, "p.cpp")
+        open(path, "w").write(probe.replace("HEADER", '"ngmlr_b200_ialignment.h"'))
+        subprocess.run(["g++", "-std=c++11", "-w", "-I", os.path.join(ROOT, "include"), "-o", os.path.join(d, "p"), path,
+                        "-Wl,--unresolved-symbols=ignore-all"], check=True)
+        out = subprocess.run([os.path.join(d, "p")], capture_output=True, text=True, check=True).stdout
+    assert out == REFERENCE_IALIGNMENT_LAYOUT, out

@@ -1,5 +1,6 @@
 """CPU tests of host-side logic: corridor geometry mirrors and batch packing."""
 import numpy as np
+import pytest
 
 from ngmlr_b200 import PackedBatch, corridor, synth
 
