@@ -292,7 +292,9 @@ int ngmlr_b200_convex_upload_windows(ngmlr_b200_ctx* ctx, int n, const uint64_t*
  * sub-reads -- ReadProvider::splitRead (src/ReadProvider.cpp:57-134): floor(len / read_part_length)
  * consecutive pieces, a read shorter than one piece is its own sub-read -- through
  * ngmlr_b200_cs_run / ngmlr_b200_cs_fetch (sub-reads in read order), and stage 4 names read parts by
- * index. Returns the number of sub-reads, or < 0. */
+ * index. Returns the number of sub-reads, or < 0.
+ * A read of at most read_part_length bases takes ngmlr's short-read path, whose candidate windows differ from the
+ * sub-reads': cs_run's scores for it are the sub-read window's; ngmlr_b200_map_short_reads computes the real ones. */
 int ngmlr_b200_reads_upload(ngmlr_b200_ctx* ctx, int n_reads, const char* const* seqs, const int32_t* lens,
                             int read_part_length);
 int64_t ngmlr_b200_reads_h2d_bytes(const ngmlr_b200_ctx* ctx);
@@ -451,6 +453,46 @@ size_t ngmlr_b200_sam_header(int n_refs, const char* const* ref_names, const uin
 int ngmlr_b200_sam_format(const ngmlr_b200_sam_options* opts, int64_t n_reads, const ngmlr_b200_sam_read* reads,
                           const ngmlr_b200_sam_aln* alns, int n_refs, const char* const* ref_names,
                           const int32_t* ref_name_lens, char* out, size_t cap, size_t* written);
+
+/* ---- reads of at most read_part_length bases: ScoreBuffer::scoreShortRead + AlignmentBuffer::processShortRead --
+ * ngmlr does not split such a read (src/ReadProvider.cpp:152-156); CS::SendToBuffer (src/CS.cpp:307-316) sends it to
+ * scoreShortRead instead of the sub-read scorer and the chaining code. cs_run scores its candidates with the sub-read
+ * window of ScoreBuffer::DoRun; the calls below compute what the short-read path computes instead.
+ *
+ * The duplicate removal of scoreShortRead (src/ScoreBuffer.cpp:225-239): the candidates [cand_start[i],
+ * cand_start[i+1]) of read i are sorted by location with the reference's std::sort call (equal locations -- the
+ * forward and reverse candidate of one bin -- keep libstdc++'s order, which decides the surviving strand), and one is
+ * kept iff lastLocation - location > read_part_length in unsigned 64-bit arithmetic (lastLocation starts at 0): after
+ * the sort, exact repeats of the previous location and a first candidate at 0 are dropped. kept[] (room for
+ * cand_start[n] entries) receives the candidate indices of the survivors in location order, read i's from
+ * kept_start[i] to kept_start[i+1]. No context: host code. Returns n or -1. */
+int ngmlr_b200_dedupe_short_read_candidates(int n, const int64_t* cand_start, const uint64_t* locs,
+                                            int read_part_length, int32_t* kept, int64_t* kept_start);
+
+/* scoreShortRead's scores (src/ScoreBuffer.cpp:245-272) for n (resident read, location, strand) pairs: read
+ * read_index[i] of ngmlr_b200_reads_upload (at most 256 bases), or its MappedRead::computeReverseSeq when
+ * reverse[i], against DecodeRefSequence(buf, 0, loc - (corridor >> 1), len + corridor) with
+ * corridor = (int)(len * 0.3 + 256) ('N' x (len + corridor) where decoding fails), StrippedSW::SingleScore semantics.
+ * Windows decoded straight from the resident genome on the device. Returns n or < 0. */
+int ngmlr_b200_score_short_reads(ngmlr_b200_ctx* ctx, int n, const int32_t* read_index, const uint64_t* locs,
+                                 const uint8_t* reverse, float* scores);
+
+/* The whole short-read path for every read of the resident batch of at most read_part_length (<= 256) bases, after
+ * ngmlr_b200_reads_upload (same read_part_length) + ngmlr_b200_cs_run: duplicate removal, scoring as
+ * ngmlr_b200_score_short_reads, order + MQ as ngmlr_b200_select_candidates (without the 0.75 cut), the alignment loop
+ * of processShortRead (src/AlignmentBuffer.cpp:2564-2639; each candidate aligned as computeAlignment(..., shortRead =
+ * true) through ngmlr_b200_compute_alignments, kept if Score > 0 and the --min-residues test passes) and
+ * SequenceProvider::convert of every kept location (src/SequenceProvider.cpp:180-205). Per resident read i:
+ * n_aln[i] = -1 for a read longer than read_part_length (not handled here: it takes the chaining path), else the
+ * number of alignments (MappedRead::Calculated), records (*alns)[first_aln[i] .. + n_aln[i]) and mapped[i] = the
+ * `mapped` argument of WriteRead (the result of the LAST convert, as coded). The records carry everything
+ * ngmlr_b200_sam_format needs except name, bases and qualities; ref_id indexes SequenceProvider's reference list,
+ * which names every contig twice (ids count both strands: pass ref_names = {c0, c0, c1, c1, ...}). Records and
+ * strings are owned by the context and stay valid until the next map_short_reads call. Returns the number of
+ * resident reads or < 0. */
+int ngmlr_b200_map_short_reads(ngmlr_b200_ctx* ctx, int read_part_length, float min_residues, int32_t* n_aln,
+                               int64_t* first_aln, int32_t* mapped, const ngmlr_b200_sam_aln** alns,
+                               int64_t* n_alns_total);
 
 #ifdef __cplusplus
 }

@@ -67,7 +67,8 @@ C_API_SYMBOLS = (
     "ngmlr_b200_compute_alignments", "ngmlr_b200_compute_alignments_stats", "ngmlr_b200_intervals_upload",
     "ngmlr_b200_sam_header", "ngmlr_b200_sam_format", "ngmlr_b200_ngm_write_index", "ngmlr_b200_ngm_read_index",
     "ngmlr_b200_ngm_write_reference", "ngmlr_b200_ngm_read_reference", "ngmlr_b200_cs_encode_reference",
-    "ngmlr_b200_cs_get_reference",
+    "ngmlr_b200_cs_get_reference", "ngmlr_b200_dedupe_short_read_candidates", "ngmlr_b200_score_short_reads",
+    "ngmlr_b200_map_short_reads",
 )
 PLUGIN_SYMBOLS = ("CreateAlignment", "DeleteAlignment", "SetAlignmentScoring")
 
@@ -143,6 +144,13 @@ def load():
                                                   C.POINTER(AlignResult), i32p]
     lib.ngmlr_b200_intervals_upload.argtypes = [vp, C.c_int, C.POINTER(Interval), C.POINTER(Anchor), C.c_int]
     lib.ngmlr_b200_compute_alignments_stats.argtypes = [vp, C.POINTER(BatchStats)]
+    lib.ngmlr_b200_dedupe_short_read_candidates.argtypes = [C.c_int, i64p, C.POINTER(C.c_uint64), C.c_int, i32p, i64p]
+    lib.ngmlr_b200_score_short_reads.argtypes = [vp, C.c_int, i32p, C.POINTER(C.c_uint64), C.POINTER(C.c_uint8),
+                                                 C.POINTER(C.c_float)]
+    lib.ngmlr_b200_debug_short_read_general_pairs.argtypes = [vp]
+    lib.ngmlr_b200_debug_short_read_general_pairs.restype = C.c_uint
+    # the records' type is samtext.SamAln (passed as an untyped pointer here: samtext imports this module)
+    lib.ngmlr_b200_map_short_reads.argtypes = [vp, C.c_int, C.c_float, i32p, i64p, i32p, C.POINTER(vp), i64p]
     lib.ngmlr_b200_sw_last_kernel_ms.argtypes = [vp]
     lib.ngmlr_b200_sw_last_kernel_ms.restype = C.c_float
     _lib = lib

@@ -426,10 +426,53 @@ class B200Aligner:
         n_sub = self._check(self.lib.ngmlr_b200_reads_upload(
             self.h, reads.n, reads.arr, reads.lens.ctypes.data_as(C.POINTER(C.c_int32)), int(read_part_length)))
         self._cs_n = n_sub
+        self._cs_reads = reads.n
         return n_sub
 
     def reads_h2d_bytes(self):
         return int(self.lib.ngmlr_b200_reads_h2d_bytes(self.h))
+
+    def score_short_reads(self, read_index, locs, reverse):
+        """ScoreBuffer::scoreShortRead's score of every (resident read, location, strand) pair -> float32[n]."""
+        ri = np.ascontiguousarray(read_index, dtype=np.int32)
+        lo = np.ascontiguousarray(locs, dtype=np.uint64)
+        rv = np.ascontiguousarray(reverse, dtype=np.uint8)
+        out = np.zeros(max(ri.size, 1), dtype=np.float32)
+        self._check(self.lib.ngmlr_b200_score_short_reads(
+            self.h, int(ri.size), ri.ctypes.data_as(C.POINTER(C.c_int32)), lo.ctypes.data_as(C.POINTER(C.c_uint64)),
+            rv.ctypes.data_as(C.POINTER(C.c_uint8)), out.ctypes.data_as(C.POINTER(C.c_float))))
+        return out[:ri.size]
+
+    def map_short_reads(self, read_part_length=256, min_residues=0.25):
+        """ngmlr's short-read path (scoreShortRead -> processShortRead -> WriteRead) for every resident read of at most
+        read_part_length bases, after reads_upload + cs_run. Returns one entry per resident read: None for a longer
+        read (it takes the chaining path), else (mapped, [samtext.Alignment]) -- with the caller's name, bases and
+        qualities a samtext.Read. ref_id indexes the reference list that names every contig twice."""
+        from .samtext import Alignment, SamAln
+        n = self._cs_reads
+        n_aln = np.zeros(max(n, 1), dtype=np.int32)
+        first = np.zeros(max(n, 1), dtype=np.int64)
+        mapped = np.zeros(max(n, 1), dtype=np.int32)
+        alns = C.c_void_p()
+        total = C.c_int64(0)
+        self._check(self.lib.ngmlr_b200_map_short_reads(
+            self.h, int(read_part_length), float(min_residues), n_aln.ctypes.data_as(C.POINTER(C.c_int32)),
+            first.ctypes.data_as(C.POINTER(C.c_int64)), mapped.ctypes.data_as(C.POINTER(C.c_int32)), C.byref(alns),
+            C.byref(total)))
+        recs = C.cast(alns, C.POINTER(SamAln))
+        out = []
+        for i in range(n):
+            if n_aln[i] < 0:
+                out.append(None)
+                continue
+            al = []
+            for k in range(int(first[i]), int(first[i]) + int(n_aln[i])):
+                a = recs[k]
+                al.append(Alignment(int(a.ref_pos), int(a.ref_id), bool(a.reverse), a.score, a.mq, a.nm, a.identity,
+                                    a.qstart, a.qend, bytes(a.cigar), bytes(a.md), a.sv_type, bool(a.primary),
+                                    bool(a.skip), a.cigar_ops))
+            out.append((bool(mapped[i]), al))
+        return out
 
     def compute_alignments(self, tasks, read_part_length=256):
         """AlignmentBuffer::computeAlignment for every task (ngmlr_b200.intervals.IntervalTask or a

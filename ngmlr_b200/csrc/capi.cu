@@ -561,6 +561,7 @@ int ngmlr_b200_cs_build_index(ngmlr_b200_ctx* ctx, const uint64_t* contig_start,
   cs->k = k;
   cs->bin_shift = bin_shift;
   cs->rn = 0;
+  cs->reads_searched = false;
   if (n_positions) *n_positions = s.n_positions;
   return 0;
 }
@@ -621,6 +622,7 @@ int ngmlr_b200_cs_search_batch(ngmlr_b200_ctx* ctx, int n, const char* const* se
   }
   cs->last_seq_off = seq_off;
   cs->rn = 0;              // d_seq / d_off / d_len are shared with the resident pipeline: invalidate it
+  cs->reads_searched = false;
   cs->seq_base = nullptr;
   std::vector<uint8_t> hseq(bytes + 16, 0);
   parallel_for(n, 256, [&](int i) { memcpy(hseq.data() + seq_off[i], seqs[i], (size_t)std::max(lens[i], 0)); });
@@ -1041,6 +1043,7 @@ int ngmlr_b200_cs_upload(ngmlr_b200_ctx* ctx, int n, const char* const* seqs, co
   cs->rbytes = bytes;
   cs->seq_base = cs->d_seq.p;
   cs->n_cand = 0;
+  cs->reads_searched = false;
   return 0;
 }
 
@@ -1171,6 +1174,7 @@ int ngmlr_b200_cs_run(ngmlr_b200_ctx* ctx, float sensitivity, float min_kmer_hit
   }
   CU(cudaEventRecord(cs->ev1, st));
   CU(nb_stream_sync(ctx, st));
+  cs->reads_searched = cs->seq_base == ctx->d_reads.p;
   if (n_candidates) *n_candidates = (int64_t)m;
   if (kernel_ms) cudaEventElapsedTime(kernel_ms, cs->ev0, cs->ev1);
   return 0;

@@ -64,6 +64,24 @@ __global__ void cs_compact_kernel(const CsCandidate* __restrict__ out, const uin
   }
 }
 
+// One thread per short-read candidate pair: ScoreBuffer::scoreShortRead's window (src/ScoreBuffer.cpp:245-265),
+// corridor = (int)(len * 0.3 + 256) in double arithmetic (no FMA contraction), window
+// DecodeRefSequence(buf, 0, loc - (corridor >> 1), len + corridor), and the whole read as the query.
+__global__ void cs_short_geometry_kernel(const int32_t* __restrict__ read_idx, const unsigned long long* __restrict__ loc,
+                                         const uint64_t* __restrict__ read_off, const int32_t* __restrict__ read_len,
+                                         int n, unsigned long long* __restrict__ win_pos, int32_t* __restrict__ win_len,
+                                         uint64_t* __restrict__ qoff, int32_t* __restrict__ qlen) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const int r = read_idx[i];
+  const int len = read_len[r];
+  const int corridor = (int)__dadd_rn(__dmul_rn((double)len, 0.3), 256.0);
+  win_pos[i] = loc[i] - (unsigned long long)(corridor >> 1);  // uloc arithmetic
+  win_len[i] = len + corridor;
+  qoff[i] = read_off[r];
+  qlen[i] = len + 1;  // strlen + 1
+}
+
 }  // namespace
 
 cudaError_t cs_exclusive_scan(void* temp, size_t& temp_bytes, const unsigned long long* in,
@@ -90,6 +108,15 @@ cudaError_t launch_cs_compact(const CsCandidate* out, const uint64_t* out_off, c
   const int warps_per_cta = 8;
   cs_compact_kernel<<<(n + warps_per_cta - 1) / warps_per_cta, warps_per_cta * 32, 0, stream>>>(
       out, out_off, out_count, cstart, seq_off, seq_len, n, half_corridor, loc, score, rev, win_pos, qoff, qlen);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_cs_short_geometry(const int32_t* read_idx, const unsigned long long* loc, const uint64_t* read_off,
+                                     const int32_t* read_len, int n, unsigned long long* win_pos, int32_t* win_len,
+                                     uint64_t* qoff, int32_t* qlen, cudaStream_t stream) {
+  if (n <= 0) return cudaSuccess;
+  cs_short_geometry_kernel<<<(n + 255) / 256, 256, 0, stream>>>(read_idx, loc, read_off, read_len, n, win_pos, win_len,
+                                                                qoff, qlen);
   return cudaGetLastError();
 }
 

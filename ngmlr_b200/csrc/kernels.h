@@ -57,9 +57,14 @@ struct SwParams {
   const unsigned long long* win_pos;
   const uint8_t* rev;
   int win_len;                 // refMaxLen (308)
+  // short-read scoring (ScoreBuffer::scoreShortRead): the window length of pair i is win_lens[i]
+  const int32_t* win_lens;
+  unsigned int* general_pairs; // optional: counts pairs of the short-read launch that miss the ungapped path
 };
 cudaError_t launch_sw_score(const SwParams& p, int grid, cudaStream_t stream);
 cudaError_t launch_sw_score_gather(const SwParams& p, int grid, cudaStream_t stream);
+// gather mode with per-pair windows of up to 640 columns (short reads: len + (int)(len * 0.3 + 256) <= 588)
+cudaError_t launch_sw_score_gather_short(const SwParams& p, int grid, cudaStream_t stream);
 
 cudaError_t launch_decode_windows(const RefDecodeParams& p, cudaStream_t stream);
 // one contig's characters (device) -> 4-bit codes, two per byte (_SequenceProvider::Init's encoding)
@@ -91,5 +96,9 @@ cudaError_t launch_cs_compact(const CsCandidate* out, const uint64_t* out_off, c
                               const unsigned long long* cstart, const uint64_t* seq_off, const int32_t* seq_len,
                               int n, int half_corridor, unsigned long long* loc, float* score, uint8_t* rev,
                               unsigned long long* win_pos, uint64_t* qoff, int32_t* qlen, cudaStream_t stream);
+// short-read candidate pairs (read index, location) -> the window and query of ScoreBuffer::scoreShortRead
+cudaError_t launch_cs_short_geometry(const int32_t* read_idx, const unsigned long long* loc, const uint64_t* read_off,
+                                     const int32_t* read_len, int n, unsigned long long* win_pos, int32_t* win_len,
+                                     uint64_t* qoff, int32_t* qlen, cudaStream_t stream);
 
 }  // namespace nb

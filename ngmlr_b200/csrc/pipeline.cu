@@ -256,6 +256,7 @@ int ngmlr_b200_reads_upload(ngmlr_b200_ctx* ctx, int n_reads, const char* const*
   cs->rbytes = bytes;
   cs->seq_base = ctx->d_reads.p;
   cs->n_cand = 0;
+  cs->reads_searched = false;
   ctx->reads_h2d_bytes = (int64_t)(bytes + ((size_t)n_reads + 1) * 8 + n_sub * 12);
   return (int)n_sub;
 }

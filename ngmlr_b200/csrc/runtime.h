@@ -281,6 +281,10 @@ struct ngmlr_b200_ctx {
   int64_t ca_h2d_bytes = 0, ca_d2h_bytes = 0, ca_cells = 0;
   float ca_fill_ms = 0, ca_traceback_ms = 0, ca_text_ms = 0;
   int ca_batches = 0;
+  // results of the last ngmlr_b200_map_short_reads call (short_reads.cu): records and the CIGAR / MD strings they
+  // point into
+  std::vector<ngmlr_b200_sam_aln> sr_alns;
+  std::vector<std::string> sr_text;
 
   // ---- sw state ----
   nb::PinBuf<uint8_t> h_sw_seq;
@@ -365,12 +369,22 @@ struct CsState {
   DevBuf<float> d_cscore;
   long long n_cand = 0;
   unsigned long long n_small_tables = 1;  // tables of the last run that live in shared memory
+  bool reads_searched = false;  // the candidates on the device are cs_run's for the sub-reads of the last reads_upload
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
   std::vector<int64_t> h_cstart;
   // pinned staging for the resident pipeline's upload / fetch
   PinBuf<uint8_t> p_seq, p_rev;
   PinBuf<float> p_score, p_sw;
   PinBuf<uint64_t> p_loc;
+  // short-read scoring (short_reads.cu): pairs (read, location, strand) -> window, query, score
+  DevBuf<int32_t> d_sr_ridx, d_sr_winlen, d_sr_qlen;
+  DevBuf<unsigned long long> d_sr_loc, d_sr_winpos;
+  DevBuf<uint64_t> d_sr_qoff;
+  DevBuf<uint8_t> d_sr_rev;
+  DevBuf<float> d_sr_sw;
+  DevBuf<unsigned int> d_sr_general;
+  DevBuf<int32_t> d_sr_scratch;
+  unsigned int sr_general_pairs = 0;  // pairs of the last short-read scoring that missed the ungapped path
 };
 
 CsState* cs_state(ngmlr_b200_ctx* ctx, bool create);

@@ -32,6 +32,9 @@ constexpr unsigned FULL = 0xffffffffu;
 constexpr int SW_ROWS = 9;  // 32 * 9 = 288 >= 257 = 256-bp sub-read + NUL: one pass for the hot case
 constexpr int SW_GAP = 255;
 constexpr int SW_COLS = 384;  // widest window of the ungapped hot path (ScoreBuffer windows: 307)
+// widest window of the short-read scorer's instantiation: scoreShortRead's windows have
+// len + (int)(len * 0.3 + 256) <= 588 characters for reads of <= 256 bases
+constexpr int SW_COLS_SHORT = 640;
 constexpr int SW_WARPS_PER_CTA = 4;
 
 __device__ __forceinline__ int nt_code(uint32_t c) {
@@ -56,7 +59,8 @@ struct GenomeWindow {
   unsigned long long pos, concat_len;
   int odd;        // position & 1: one extra leading base
   int pairs2;     // 2 * ceil(len / 2) characters decoded pairwise
-  int x_at;       // index (after the odd base) that is overwritten by 'x' when len is odd, else -1
+  int x_at;       // index (after the odd base) that is overwritten by 'x' when len is odd, else pairs2 (none: the
+                  // odd leading base has index -1)
   int str_len;    // strlen of the decoded window
   bool invalid;   // position >= concat_len: the caller fills the buffer with 'N'
   __device__ void init(const uint8_t* e, unsigned long long p, unsigned long long cl, int buffer_len) {
@@ -66,7 +70,7 @@ struct GenomeWindow {
     if (!invalid && p + len > cl) { end = p + len - cl; len -= end; }
     odd = (int)(p & 1ull);
     pairs2 = (int)(((len + 1) / 2) * 2);
-    x_at = (len & 1ull) ? pairs2 - 1 : -1;
+    x_at = (len & 1ull) ? pairs2 - 1 : pairs2;
     str_len = invalid ? buffer_len : odd + pairs2 + (int)end;
   }
   __device__ __forceinline__ int code(int i) const {
@@ -158,13 +162,14 @@ __device__ __forceinline__ float sw_ungapped(const GenomeWindow& gw, const uint8
   return (float)(best & 0xffff);
 }
 
-template <bool GATHER>
+// COLS: widest window of the ungapped path (shared table size); PAIR_WIN: window lengths per pair (p.win_lens)
+template <bool GATHER, int COLS, bool PAIR_WIN>
 __global__ void __launch_bounds__(SW_WARPS_PER_CTA * 32) sw_score_kernel(const SwParams p) {
   const int lane = threadIdx.x & 31;
   const int warp_global = blockIdx.x * SW_WARPS_PER_CTA + (threadIdx.x >> 5);
   const int nwarps = gridDim.x * SW_WARPS_PER_CTA;
   int2* strip = reinterpret_cast<int2*>(p.scratch) + (size_t)warp_global * p.scratch_stride;
-  __shared__ uint32_t s_tab[SW_WARPS_PER_CTA][SW_COLS + 64];
+  __shared__ uint32_t s_tab[SW_WARPS_PER_CTA][COLS + 64];
   // 0 the compiler cannot see through: keeps the RELU floor of the packed ops in one register
   // (a literal 0 is re-materialised with a PRMT per use)
   const uint32_t zero = (uint32_t)p.n >> 31;
@@ -173,7 +178,7 @@ __global__ void __launch_bounds__(SW_WARPS_PER_CTA * 32) sw_score_kernel(const S
     GenomeWindow gw;
     int rlen_g = 0;
     if (GATHER) {
-      gw.init(p.enc, p.win_pos[pair], p.concat_len, p.win_len);
+      gw.init(p.enc, p.win_pos[pair], p.concat_len, PAIR_WIN ? p.win_lens[pair] : p.win_len);
       rlen_g = gw.str_len + 1;  // strlen + 1: the NUL is scored
     }
     const bool q_rev = GATHER && p.rev[pair];
@@ -185,17 +190,18 @@ __global__ void __launch_bounds__(SW_WARPS_PER_CTA * 32) sw_score_kernel(const S
     const uint8_t* __restrict__ ref = GATHER ? p.seq : p.seq + p.ref_off[pair];
     const uint8_t* __restrict__ qry = p.seq + p.qry_off[pair];
     int best = 0;
-    // ---- hot case: at most 320 query characters (256-bp sub-read + NUL), window of <= 384 columns ----
+    // ---- hot case: at most 320 query characters (256-bp sub-read + NUL), window of <= COLS columns ----
     // A gap costs 255 per base, so a gapped path beats its best ungapped piece only if it gains
     // more than 255 before AND after the gap: impossible with fewer than 512 query characters.
     // Then E and F never influence the maximum and the recurrence is H = max(0, diag + s).
-    if (qlen - 1 <= 64 * 5 && rlen - 1 <= SW_COLS) {
+    if (qlen - 1 <= 64 * 5 && rlen - 1 <= COLS) {
       const float r = (qlen - 1 <= 64 * 4)
                           ? sw_ungapped<4, GATHER>(gw, ref, qry, qlen - 1, rlen - 1, q_rev, s_tab[threadIdx.x >> 5], lane, zero)
                           : sw_ungapped<5, GATHER>(gw, ref, qry, qlen - 1, rlen - 1, q_rev, s_tab[threadIdx.x >> 5], lane, zero);
       if (lane == 0) p.out[pair] = r;
       continue;
     }
+    if (PAIR_WIN && p.general_pairs && lane == 0) atomicAdd(p.general_pairs, 1u);
     const int rows_per_pass = 32 * SW_ROWS;
     for (int row_base = 0; row_base < qlen; row_base += rows_per_pass) {
       const bool first_pass = row_base == 0;
@@ -269,13 +275,19 @@ __global__ void __launch_bounds__(SW_WARPS_PER_CTA * 32) sw_score_kernel(const S
 
 cudaError_t launch_sw_score(const SwParams& p, int grid, cudaStream_t stream) {
   if (p.n <= 0) return cudaSuccess;
-  sw_score_kernel<false><<<grid, SW_WARPS_PER_CTA * 32, 0, stream>>>(p);
+  sw_score_kernel<false, SW_COLS, false><<<grid, SW_WARPS_PER_CTA * 32, 0, stream>>>(p);
   return cudaGetLastError();
 }
 
 cudaError_t launch_sw_score_gather(const SwParams& p, int grid, cudaStream_t stream) {
   if (p.n <= 0) return cudaSuccess;
-  sw_score_kernel<true><<<grid, SW_WARPS_PER_CTA * 32, 0, stream>>>(p);
+  sw_score_kernel<true, SW_COLS, false><<<grid, SW_WARPS_PER_CTA * 32, 0, stream>>>(p);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_sw_score_gather_short(const SwParams& p, int grid, cudaStream_t stream) {
+  if (p.n <= 0) return cudaSuccess;
+  sw_score_kernel<true, SW_COLS_SHORT, true><<<grid, SW_WARPS_PER_CTA * 32, 0, stream>>>(p);
   return cudaGetLastError();
 }
 
