@@ -383,6 +383,43 @@ int ngmlr_b200_ngm_write_reference(const char* path, const uint8_t* bin_ref, uin
 int ngmlr_b200_ngm_read_reference(const char* path, uint32_t* n_refs, uint64_t* used_bytes, uint64_t* alloc_bytes,
                                   uint64_t* seq_start, uint32_t* seq_len, char* names, uint8_t* bin_ref);
 
+/* ---- ngmlr's start-up in one call: _SequenceProvider::Init + the CompactPrefixTable constructor ------------------
+ * (src/SequenceProvider.cpp:246-424, src/PrefixTable.cpp:97-128), with the encoding and the k-mer index built on the
+ * device. In ngmlr's order:
+ *   - <fasta>-enc.2.ngm exists: it is read and installed (ngmlr_b200_ngm_read_reference -> cs_set_reference +
+ *     set_ref_starts); an invalid one is an error, as in ngmlr. Otherwise the FASTA / FASTQ file (plain or gzip) is
+ *     read as ngmlr's kseq_read loop reads it, encoded on the device (cs_encode_reference) and the file is written
+ *     unless skip_write.
+ *   - <fasta>-ht-<k>-<kmer_skip>.2.ngm exists and is a valid single-unit table for k / kmer_skip: it is read and
+ *     installed (cs_set_index). Otherwise the index is built on the device (cs_build_index) and written unless
+ *     skip_write. A table ngmlr would reject (wrong cookie, k or skip; ngmlr stops there) is rebuilt as well.
+ *   - rebuild = 1 ignores both files.
+ * Caches are written under a temporary name and renamed; a cache that cannot be written is skipped (ngmlr warns and
+ * goes on) and its flag stays clear. Genomes of more than 0xffff0000 - 1 positions (more than one table unit of the
+ * reference's index) or with more k-mer callbacks than 2^31 are refused. On success the context holds the reference,
+ * refStartPos and the index, ready for reads_upload -> cs_run; on failure it keeps what it held when the failure is
+ * found before anything reaches the device (missing / unreadable / empty / oversized input) and holds no reference
+ * and no index otherwise. opts NULL: k 13, kmer_skip 2, bin_shift 4, max_prefix_freq 1000, write, no rebuild.
+ * *n_contigs = contigs kept (more than 10 bases), *concat_len = GetConcatRefLen(), *flags = NGMLR_B200_LOAD_* bits.
+ * Returns 0 or < 0 (ngmlr_b200_last_error). */
+typedef struct {
+  int32_t k, kmer_skip, bin_shift, max_prefix_freq;
+  int32_t skip_write;
+  int32_t rebuild;
+} ngmlr_b200_reference_options;
+#define NGMLR_B200_LOAD_REFERENCE_READ 1    /* <fasta>-enc.2.ngm was read */
+#define NGMLR_B200_LOAD_REFERENCE_WRITTEN 2 /* <fasta>-enc.2.ngm was written */
+#define NGMLR_B200_LOAD_INDEX_READ 4        /* <fasta>-ht-<k>-<skip>.2.ngm was read */
+#define NGMLR_B200_LOAD_INDEX_WRITTEN 8     /* <fasta>-ht-<k>-<skip>.2.ngm was written */
+int ngmlr_b200_load_reference(ngmlr_b200_ctx* ctx, const char* fasta_path, const ngmlr_b200_reference_options* opts,
+                              int32_t* n_contigs, uint64_t* concat_len, int32_t* flags);
+/* The contig table of the last load_reference: per kept contig its name (cut to 100 characters as RefIdx::name,
+ * name_lens[i] characters, NUL terminated; valid until the context's reference changes), SeqStart and SeqLen.
+ * SAM writers name contig i twice (SequenceProvider's ids count both strands). Arrays may be NULL. Returns the number
+ * of contigs, or < 0 when the context's reference did not come from load_reference. */
+int ngmlr_b200_reference_contigs(ngmlr_b200_ctx* ctx, const char** names, int32_t* name_lens, uint64_t* starts,
+                                 uint64_t* lens);
+
 /* ---- SAM text (SURVEY section 8(f)4) ----------------------------------------------------------
  * Replaces SAMWriter::DoWriteProlog / DoWriteRead -> DoWriteReadGeneric / DoWriteUnmappedRead
  * (src/SAMWriter.cpp:22-85, 87-224, 301-363) and the per-read loop of GenericReadWriter::WriteRead

@@ -68,8 +68,15 @@ C_API_SYMBOLS = (
     "ngmlr_b200_sam_header", "ngmlr_b200_sam_format", "ngmlr_b200_ngm_write_index", "ngmlr_b200_ngm_read_index",
     "ngmlr_b200_ngm_write_reference", "ngmlr_b200_ngm_read_reference", "ngmlr_b200_cs_encode_reference",
     "ngmlr_b200_cs_get_reference", "ngmlr_b200_dedupe_short_read_candidates", "ngmlr_b200_score_short_reads",
-    "ngmlr_b200_map_short_reads",
+    "ngmlr_b200_map_short_reads", "ngmlr_b200_load_reference", "ngmlr_b200_reference_contigs",
 )
+
+# flags of ngmlr_b200_load_reference (include/ngmlr_b200.h)
+LOAD_REFERENCE_READ, LOAD_REFERENCE_WRITTEN, LOAD_INDEX_READ, LOAD_INDEX_WRITTEN = 1, 2, 4, 8
+
+
+class ReferenceOptions(C.Structure):
+    _fields_ = [(k, C.c_int32) for k in ("k", "kmer_skip", "bin_shift", "max_prefix_freq", "skip_write", "rebuild")]
 PLUGIN_SYMBOLS = ("CreateAlignment", "DeleteAlignment", "SetAlignmentScoring")
 
 _lib = None
@@ -151,6 +158,11 @@ def load():
     lib.ngmlr_b200_debug_short_read_general_pairs.restype = C.c_uint
     # the records' type is samtext.SamAln (passed as an untyped pointer here: samtext imports this module)
     lib.ngmlr_b200_map_short_reads.argtypes = [vp, C.c_int, C.c_float, i32p, i64p, i32p, C.POINTER(vp), i64p]
+    lib.ngmlr_b200_load_reference.argtypes = [vp, C.c_char_p, C.POINTER(ReferenceOptions), i32p, u64p, i32p]
+    lib.ngmlr_b200_reference_contigs.argtypes = [vp, cpp, i32p, u64p, u64p]
+    lib.ngmlr_b200_load_reference_ms.argtypes = [vp, C.POINTER(C.c_float)]
+    lib.ngmlr_b200_debug_read_fasta.argtypes = [C.c_char_p, C.c_uint64, i64p, u64p, u64p, u64p, i64p, u64p, C.c_char_p,
+                                                C.c_char_p, C.c_char_p, C.c_int]
     lib.ngmlr_b200_sw_last_kernel_ms.argtypes = [vp]
     lib.ngmlr_b200_sw_last_kernel_ms.restype = C.c_float
     _lib = lib

@@ -11,6 +11,7 @@ All compute happens in the CUDA library; nothing here (or anywhere in the packag
 alignment on the CPU.
 """
 import ctypes as C
+import os
 from dataclasses import dataclass, field
 
 import numpy as np
@@ -18,6 +19,27 @@ import numpy as np
 from . import _lib
 
 DEFAULT_SCORING = (2.0, -5.0, -5.0, -5.0, -1.0, 0.15)
+
+
+@dataclass
+class LoadedReference:
+    """What B200Aligner.load_reference installed: the contig table of SequenceProvider (kept contigs, names cut to
+    100 characters; SAM writers list every contig twice), which cache files were read or written, and the phase times
+    in milliseconds (host clock around work that ends in a device synchronise)."""
+    PHASES = ("read", "install", "reference_write", "index", "index_write", "total")
+    names: list
+    starts: list
+    lens: list
+    concat_len: int
+    reference_read: bool
+    reference_written: bool
+    index_read: bool
+    index_written: bool
+    ms: dict
+
+    def sam_ref_names(self):
+        """The reference list SAM records index (ids count both strands): every name twice."""
+        return [n for n in self.names for _ in (0, 1)]
 
 
 @dataclass
@@ -329,6 +351,32 @@ class B200Aligner:
                                                              None))
         return EncodedReference(enc, int(cl.value), [int(ks[i]) for i in range(kept.value)],
                                 [int(kl[i]) for i in range(kept.value)])
+
+    def load_reference(self, path, k=13, kmer_skip=2, bin_shift=4, skip_write=False, rebuild=False, max_prefix_freq=1000):
+        """ngmlr's start-up (ngmlr_b200_load_reference): the reference and its k-mer index from <path>-enc.2.ngm and
+        <path>-ht-<k>-<kmer_skip>.2.ngm where they exist, else from the FASTA / FASTQ file (plain or gzip) with the
+        encoding and the index built on the device and both caches written next to it (unless skip_write). Installs
+        the reference, refStartPos and the index in this context. Returns a LoadedReference: the contig table (names
+        cut to 100 characters, SeqStart, SeqLen), which cache files were read / written, and the phase times."""
+        opts = _lib.ReferenceOptions(k, kmer_skip, bin_shift, max_prefix_freq, int(bool(skip_write)), int(bool(rebuild)))
+        n, cl, fl = C.c_int32(0), C.c_uint64(0), C.c_int32(0)
+        self._check(self.lib.ngmlr_b200_load_reference(self.h, os.fsencode(path), C.byref(opts), C.byref(n),
+                                                       C.byref(cl), C.byref(fl)))
+        names = (C.c_char_p * n.value)()
+        nlen = np.zeros(n.value, dtype=np.int32)
+        starts = np.zeros(n.value, dtype=np.uint64)
+        lens = np.zeros(n.value, dtype=np.uint64)
+        u64p = C.POINTER(C.c_uint64)
+        self._check(self.lib.ngmlr_b200_reference_contigs(self.h, names, nlen.ctypes.data_as(C.POINTER(C.c_int32)),
+                                                          starts.ctypes.data_as(u64p), lens.ctypes.data_as(u64p)))
+        ms = (C.c_float * 6)()
+        self._check(self.lib.ngmlr_b200_load_reference_ms(self.h, ms))
+        f = fl.value
+        return LoadedReference([names[i][:int(nlen[i])] for i in range(n.value)], [int(x) for x in starts],
+                               [int(x) for x in lens], int(cl.value),
+                               bool(f & _lib.LOAD_REFERENCE_READ), bool(f & _lib.LOAD_REFERENCE_WRITTEN),
+                               bool(f & _lib.LOAD_INDEX_READ), bool(f & _lib.LOAD_INDEX_WRITTEN),
+                               dict(zip(LoadedReference.PHASES, [float(x) for x in ms])))
 
     def set_reference(self, ref):
         """ref: ngmlr_b200.refindex.EncodedReference (the reference's 4-bit `binRef`)."""

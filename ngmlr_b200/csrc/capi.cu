@@ -500,6 +500,9 @@ int ngmlr_b200_cs_build_index(ngmlr_b200_ctx* ctx, const uint64_t* contig_start,
   if (k < 1 || k > 15) return ctx->fail("cs_build_index: k must be in 1..15");
   if (n_contigs < 1 || kmer_skip < 0 || max_prefix_freq < 1) return ctx->fail("cs_build_index: bad arguments");
   if (cs->concat_len >= 0xffff0000ull) return ctx->fail("cs_build_index: one table unit holds < 4 G positions");
+  if (!index_build_fits(cs->concat_len, n_contigs, kmer_skip))
+    return ctx->fail("cs_build_index: %llu positions give more k-mer callbacks than the build sorts (2^31) at kmer_skip %d",
+                     (unsigned long long)cs->concat_len, kmer_skip);
   for (int i = 0; i < n_contigs; ++i) {
     if (i && contig_start[i] < contig_start[i - 1] + contig_len[i - 1]) return ctx->fail("cs_build_index: contigs must be sorted and disjoint");
     if (contig_start[i] + contig_len[i] > cs->concat_len) return ctx->fail("cs_build_index: contig %d leaves the reference", i);
@@ -751,6 +754,7 @@ int ngmlr_b200_cs_set_reference(ngmlr_b200_ctx* ctx, const uint8_t* bin_ref, uin
   CU(nb_stream_sync(ctx, ctx->stream));
   cs->enc_bytes = n_bytes;
   cs->concat_len = concat_len;
+  cs->contig_names.clear();  // no longer the contigs of a load_reference
   return 0;
 }
 
@@ -803,6 +807,7 @@ int ngmlr_b200_cs_encode_reference(ngmlr_b200_ctx* ctx, int n_contigs, const cha
   CU(nb_stream_sync(ctx, ctx->stream));
   cs->enc_bytes = bytes;
   cs->concat_len = bytes * 2 - 1;
+  cs->contig_names.clear();  // no longer the contigs of a load_reference
   if (n_kept) *n_kept = (int32_t)which.size();
   for (size_t j = 0; j < which.size(); ++j) {
     if (kept_start) kept_start[j] = starts[j];

@@ -233,7 +233,8 @@ struct MaxOp {
 }  // namespace
 
 // Scratch sizes are those of a 3 Gb genome at most: concat_len * (4 + 1 + 4) bytes for the scans plus
-// 5 x 4 bytes per callback (~ concat_len / (skip + 1)) -- about 45 GB of the 180 GB for a human genome.
+// 5 x 4 bytes per callback (~ concat_len / (skip + 1)). Measured for a 3 Gb genome on an H100 80GB HBM3 (700 W):
+// 51.8 GB of device memory in use at the peak of ngmlr_b200_load_reference (DESIGN.md 4.6).
 cudaError_t build_kmer_index(const IndexBuildParams& p, IndexBuildScratch& s, cudaStream_t st) {
 #define IB(call)                      \
   do {                                \
@@ -244,6 +245,8 @@ cudaError_t build_kmer_index(const IndexBuildParams& p, IndexBuildScratch& s, cu
   const int grid = current_device_sms() * 16;
   const uint32_t n_kmers = 1u << (2 * p.k);
   const long long cl = (long long)p.concat_len;  // 64-bit item counts: a human genome has > 2^31 bases
+  // positions are scanned as uint32 and the callbacks sorted with an int item count
+  if (p.concat_len > INDEX_MAX_CONCAT_LEN || s.cb_capacity > 0x7fffffffull) return cudaErrorInvalidValue;
   // ---- 1. callbacks ----
   index_nmark_kernel<<<grid, threads, 0, st>>>(p, s.lastn);
   size_t tmp = s.cub_bytes;
@@ -260,6 +263,7 @@ cudaError_t build_kmer_index(const IndexBuildParams& p, IndexBuildScratch& s, cu
   const unsigned long long n_cb = (unsigned long long)last_slot + last_flag;
   s.n_callbacks = n_cb;
   if (n_cb > s.cb_capacity) return cudaErrorMemoryAllocation;
+  if (n_cb > 0x7fffffffull) return cudaErrorInvalidValue;
   index_emit_kernel<<<grid, threads, 0, st>>>(p, s.flag, s.slot, s.prefix, s.pos);
   // ---- 2 + 3. repeat filter, frequencies ----
   IB(cudaMemsetAsync(s.freq, 0, (size_t)(n_kmers + 1) * 4, st));

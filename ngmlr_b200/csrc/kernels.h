@@ -85,6 +85,15 @@ cudaError_t launch_unpack_index(const uint8_t* packed, uint32_t n, uint32_t* tab
 // k-mer index of the resident encoded reference, built on the device (cs_index_build.cu)
 cudaError_t build_kmer_index(const IndexBuildParams& p, IndexBuildScratch& s, cudaStream_t stream);
 size_t index_build_cub_bytes(unsigned long long concat_len, unsigned long long max_callbacks, int k);
+// Positions of the genome (< 0xffff0000: one table unit, 32-bit scans) and k-mer callbacks (the radix sort's int item
+// count) that build_kmer_index can handle; it refuses anything larger with cudaErrorInvalidValue.
+constexpr unsigned long long INDEX_MAX_CONCAT_LEN = 0xffff0000ull - 1;
+inline unsigned long long index_callback_capacity(unsigned long long concat_len, int n_contigs, int kmer_skip) {
+  return concat_len / (unsigned long long)(kmer_skip + 1) + (unsigned long long)n_contigs * 64 + 1024;
+}
+inline bool index_build_fits(unsigned long long concat_len, int n_contigs, int kmer_skip) {
+  return concat_len <= INDEX_MAX_CONCAT_LEN && index_callback_capacity(concat_len, n_contigs, kmer_skip) <= 0x7fffffffull;
+}
 
 // device-resident candidate pipeline glue (cs_pipeline.cu)
 cudaError_t cs_exclusive_scan(void* temp, size_t& temp_bytes, const unsigned long long* in,

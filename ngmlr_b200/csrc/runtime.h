@@ -385,6 +385,12 @@ struct CsState {
   DevBuf<unsigned int> d_sr_general;
   DevBuf<int32_t> d_sr_scratch;
   unsigned int sr_general_pairs = 0;  // pairs of the last short-read scoring that missed the ungapped path
+  // the contig table of the last ngmlr_b200_load_reference (reference_load.cu); cleared when another call replaces
+  // the reference
+  std::vector<std::string> contig_names;
+  std::vector<const char*> contig_name_ptrs;
+  std::vector<uint64_t> contig_start, contig_len;
+  float load_ms[6] = {0, 0, 0, 0, 0, 0};  // read / parse, install, reference write, index, index write, total
 };
 
 CsState* cs_state(ngmlr_b200_ctx* ctx, bool create);
