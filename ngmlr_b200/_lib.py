@@ -106,6 +106,8 @@ def load():
     lib.ngmlr_b200_set_fill_ctas_per_sm.argtypes = [vp, C.c_int]
     lib.ngmlr_b200_set_small_batch_teams.argtypes = [vp, C.c_int]
     lib.ngmlr_b200_debug_set_arena_words.argtypes = [vp, C.c_longlong]
+    lib.ngmlr_b200_debug_rampfree_problems.argtypes = [vp]
+    lib.ngmlr_b200_debug_rampfree_problems.restype = C.c_longlong
     lib.ngmlr_b200_debug_set_big_team.argtypes = [vp, C.c_longlong, C.c_int]
     batch = [vp, C.c_int, cpp, i32p, cpp, i32p, i32p, i32p, i64p, i32p, i32p]
     lib.ngmlr_b200_convex_upload.argtypes = batch

@@ -570,6 +570,10 @@ class B200Aligner:
         """Test hook: initial size of the direction arena (-1 = the host's estimate)."""
         self.lib.ngmlr_b200_debug_set_arena_words(self.h, int(words))
 
+    def debug_rampfree_problems(self):
+        """Test hook: problems filled by the ramp-free fill kernel since the context was created."""
+        return int(self.lib.ngmlr_b200_debug_rampfree_problems(self.h))
+
     def set_small_batch_teams(self, on):
         """16-warp teams for batches of at most one problem per SM (default on); see ngmlr_b200_set_small_batch_teams."""
         self.lib.ngmlr_b200_set_small_batch_teams(self.h, int(bool(on)))

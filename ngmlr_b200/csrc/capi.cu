@@ -99,12 +99,14 @@ int ngmlr_b200_create(int gpu_id, const ngmlr_b200_scoring* s, ngmlr_b200_ctx** 
   // the context's stream (candidate search, traceback, text, copies) outranks its fill launches
   cudaStreamCreateWithPriority(&ctx->stream, cudaStreamNonBlocking, prio_greatest);
   cudaStreamCreateWithPriority(&ctx->stream2, cudaStreamNonBlocking, prio_least);
+  cudaStreamCreateWithPriority(&ctx->stream3, cudaStreamNonBlocking, prio_least);
   cudaStreamCreateWithPriority(&ctx->stream_fill, cudaStreamNonBlocking, prio_least);
   cudaEventCreateWithFlags(&ctx->ev_fill, cudaEventDisableTiming);
   if (const char* e = getenv("NGMLR_B200_FILL_PERSISTENT")) ctx->fill_persistent = atoi(e);
   if (const char* e = getenv("NGMLR_B200_SMALL_BATCH_BIG_TEAMS")) ctx->small_batch_big_teams = atoi(e);
   if (const char* e = getenv("NGMLR_B200_FILL_RESIDENT")) ctx->fill_resident = std::max(0, atoi(e));
   cudaEventCreateWithFlags(&ctx->ev_big, cudaEventDisableTiming);
+  cudaEventCreateWithFlags(&ctx->ev_team, cudaEventDisableTiming);
   cudaEventCreateWithFlags(&ctx->ev_sync, cudaEventDisableTiming | cudaEventBlockingSync);
   if (const char* e = getenv("NGMLR_B200_SPIN_SYNC")) ctx->spin_sync = atoi(e) != 0;
   for (auto& ev : ctx->ev) cudaEventCreate(&ev);
@@ -119,6 +121,17 @@ int ngmlr_b200_create(int gpu_id, const ngmlr_b200_scoring* s, ngmlr_b200_ctx** 
   ctx->sc.decay = d.gap_decay;
   ctx->raw = scoring_needs_raw(ctx->sc);
   if (const char* e = getenv("NGMLR_B200_FILL_TEAM")) ctx->force_team = atoi(e);
+  if (const char* e = getenv("NGMLR_B200_FILL_SCHEDULE")) {
+    if (!strcmp(e, "ramped")) ctx->fill_schedule = 0;
+    else if (!strcmp(e, "rampfree")) ctx->fill_schedule = 1;
+    else if (!strcmp(e, "rampfree-all")) ctx->fill_schedule = 2;
+    else {
+      g_create_error = std::string("ngmlr_b200: NGMLR_B200_FILL_SCHEDULE=") + e + ": expected ramped, rampfree or rampfree-all";
+      ngmlr_b200_destroy(ctx);
+      return -1;
+    }
+  }
+  if (const char* e = getenv("NGMLR_B200_RF_TEAM_CELLS")) ctx->rf_team_cells = strtoull(e, nullptr, 10);
   if (const char* e = getenv("NGMLR_B200_FILL_CTAS_PER_SM")) ctx->fill_ctas_cap = std::max(0, atoi(e));
   if (const char* e = getenv("NGMLR_B200_NO_CORRIDOR_PACKING")) ctx->no_corridor_packing = atoi(e);
   *out = ctx;
@@ -142,8 +155,10 @@ void ngmlr_b200_destroy(ngmlr_b200_ctx* ctx) {
   ctx->d_sw_scratch.release();
   for (auto& ev : ctx->ev) cudaEventDestroy(ev);
   if (ctx->ev_big) cudaEventDestroy(ctx->ev_big);
+  if (ctx->ev_team) cudaEventDestroy(ctx->ev_team);
   if (ctx->ev_sync) cudaEventDestroy(ctx->ev_sync);
   if (ctx->stream2) cudaStreamDestroy(ctx->stream2);
+  if (ctx->stream3) cudaStreamDestroy(ctx->stream3);
   if (ctx->stream_fill) cudaStreamDestroy(ctx->stream_fill);
   if (ctx->ev_fill) cudaEventDestroy(ctx->ev_fill);
   if (ctx->own_stream && ctx->stream) cudaStreamDestroy(ctx->stream);
@@ -221,6 +236,9 @@ int ngmlr_b200_debug_set_big_team(ngmlr_b200_ctx* ctx, long long cells, int widt
   ctx->big_width = width;
   return 0;
 }
+
+// Test hook: problems filled by the ramp-free kernel since the context was created.
+long long ngmlr_b200_debug_rampfree_problems(ngmlr_b200_ctx* ctx) { return ctx ? (long long)ctx->rf_problems : -1; }
 
 // force_team: -1 auto, 0 one warp per problem, 1 four-warp teams. Test / tuning hook.
 int ngmlr_b200_set_force_team(ngmlr_b200_ctx* ctx, int v) {

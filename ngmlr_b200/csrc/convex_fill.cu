@@ -115,6 +115,163 @@ struct TeamBest {
   unsigned long long cells;
 };
 
+// What one lane carries from step to step.
+struct LaneState {
+  // What this lane hands down / keeps for its right neighbour. EMPTY = {0, 0, STOP}.
+  // oP: scalar kernel = the I-run length as a float (0 unless the cell is an insertion);
+  //     RAW kernel    = indelRun (low 16 bits) | direction << 16.
+  float oS, oU;
+  uint32_t oP, oC;
+  float dS;     // score of (x-1, y-1)
+  float lL;     // left_cell contribution of (x-1, y)
+  float lRunF;  // scalar kernel: D-run length of (x-1, y), 0 unless it is a deletion
+  bool lIsD;
+  int lRun;     // RAW kernel: raw indelRun / direction of (x-1, y)
+  uint32_t lDir;
+  float kS;     // best score of the current row so far (strictly above the lane's earlier best)
+  int kStep;    // step at which it was reached, -1: none
+  int rel;      // x - xlo of the current step; inside the corridor iff (unsigned)rel < rlen
+};
+
+// 16 steps of one lane: cells (x, y) with x = the lane's column at step 16 g + k. `iop` and `dwp` address the
+// chunk's staging records and the lane's direction word of group 0. ALL_ACTIVE: every lane of the warp stays
+// inside its corridor row for all 16 steps (no masking at all: the common case away from a block's wavefront ends).
+// SELF_REF (ramp-free kernel, masked groups): a lane outside its row takes the reference byte of its column
+// (step - colbase) from ref (columns outside [0, ref_len) read the padding byte ref[ref_len]) instead of from the
+// lane above.
+template <bool RAW, bool ALL_ACTIVE, int GPC, bool SELF_REF = false>
+__device__ __forceinline__ void fill_group(LaneState& st, const Scoring& sc, uint4* const io_s, uint32_t* const dwp,
+                                           const int g, const unsigned rlen, const uint32_t q, const int t0rel,
+                                           const bool is0, const bool is31, const int src_lane,
+                                           const uint8_t* ref = nullptr, int colbase = 0, unsigned ref_len = 0) {
+  uint4* iop = io_s + ((g % GPC) << 5);  // [0] lane 0's input of this step, [1] lane 31's output
+  uint32_t dw = 0;
+  {
+#pragma unroll 2  // 2 keeps the per-step predicates in registers; 4 makes ptxas spill them to a bit mask
+    for (int k = 0; k < 16; ++k) {
+      const int s = (g << 4) + k;
+      uint4 v;
+#if FILL_LANE0_LDS
+      // lanes 1..31 take their upper neighbour's cell from lane t-1, lane 0 from the staged strip record
+      v.x = __float_as_uint(__shfl_up_sync(FULL, st.oS, 1));
+      v.y = __float_as_uint(__shfl_up_sync(FULL, st.oU, 1));
+      v.z = __shfl_up_sync(FULL, st.oP, 1);
+      v.w = __shfl_up_sync(FULL, st.oC, 1);
+      if (is0) v = iop[0];
+#else
+      v.x = __float_as_uint(__shfl_sync(FULL, st.oS, src_lane));
+      v.y = __float_as_uint(__shfl_sync(FULL, st.oU, src_lane));
+      v.z = __shfl_sync(FULL, st.oP, src_lane);
+      v.w = __shfl_sync(FULL, st.oC, src_lane);
+#endif
+      const float nS = __uint_as_float(v.x), nU = __uint_as_float(v.y);
+      const bool act = ALL_ACTIVE ? true : ((unsigned)st.rel < rlen);
+      uint32_t r = v.w;
+      if (SELF_REF && !act) r = __ldg(ref + min((unsigned)(s - colbase), ref_len));
+      float dg = __fadd_rn(st.dS, sc.mis);
+      if (r == q) dg = __fadd_rn(st.dS, sc.mat);
+      st.dS = nS;
+      // Outside the corridor the cell must degenerate to {0, 0, STOP}: a NaN maximum makes every
+      // equality below false, and fmaxf(NaN, 0) = 0 gives the score.
+      const float m0 = fmaxf(fmaxf(fmaxf(st.lL, 0.0f), dg), nU);
+      const float m = (ALL_ACTIVE || act) ? m0 : __int_as_float(0x7fffffff);
+      const bool eL = (m == st.lL), eU = (m == nU), eG = (m == dg);
+      const float S = ALL_ACTIVE ? m : fmaxf(m, 0.0f);  // STOP implies m == 0
+      uint32_t code;
+      float U, L;
+      if (RAW) {
+        const uint32_t nP = v.z;
+        const int upRaw = (int)(short)(nP & 0xffffu);
+        const uint32_t upDir = (nP >> 16) & 3u;
+        const bool rawHere = st.rel < t0rel;
+        const int upRun = (rawHere || upDir == DIR_I) ? upRaw : 0;
+        const int leftRun = (rawHere || st.lDir == DIR_D) ? st.lRun : 0;
+        // priority (:1232-1267): continue D, continue I, diagonal, open D, open I, STOP
+        const bool dc = eL && (leftRun > 0);
+        const bool ic = !dc && eU && (upRun > 0);
+        const bool gg = !dc && !ic && eG;
+        const bool resolved = dc || ic || gg;
+        const bool isD = dc || (!resolved && eL);
+        const bool isI = ic || (!resolved && !eL && eU);
+        int run = dc ? leftRun : (ic ? upRun : 0);
+        run = (isD || isI) ? run + 1 : 0;
+        run = (int)(short)run;  // MatrixElement::indelRun is a short
+        code = gg ? DIR_DIAG : (isI ? DIR_I : (isD ? DIR_D : DIR_STOP));
+        // what the neighbours will see: S + min(ext_min, gap_ext + run*decay), 0 if S == 0 (:666-676)
+        const float pen = fminf(sc.ext_min, __fadd_rn(sc.gap_ext, __fmul_rn((float)run, sc.decay)));
+        float e = __fadd_rn(S, pen);
+        if (S == 0.0f) e = 0.0f;
+        U = isI ? e : __fadd_rn(S, sc.open_read);
+        L = isD ? e : __fadd_rn(S, sc.open_ref);
+        st.oP = (code << 16) | ((uint32_t)run & 0xffffu);
+        st.lRun = run;
+        st.lDir = code;
+      } else {
+        // Same priority chain as a 3-input predicate network (verified exhaustively):
+        //   D  <=>  eL && (lr || !((eU && ur) || eG))
+        //   I  <=>  !D && eU && (ur || !eG)
+        // with run lengths kept as floats (exact below 2^24; rows are < 32768 wide here).
+        const float upRunF = __uint_as_float(v.z);
+        const bool lr = st.lIsD, ur = upRunF > 0.0f;  // the left cell's run is > 0 iff it is a deletion
+        const bool X = (eU & ur) | eG;  // bitwise on purpose: straight PLOP3s, no short-circuit
+        const bool pD = eL & (lr | !X);
+        const bool pI = (!pD) & eU & (ur | !eG);
+        code = eG ? DIR_DIAG : DIR_STOP;
+        if (pI) asm volatile("mad.lo.u32 %0, %1, 0, 1;" : "=r"(code) : "r"(code));
+        if (pD) asm volatile("mad.lo.u32 %0, %1, 0, 2;" : "=r"(code) : "r"(code));
+        // at most one of the two run counters is alive after this cell
+        // "zero, then an addition under the predicate" instead of add + select: the selects, compares and
+        // min/max of this loop all go through the half-rate ALU pipe, which is what binds the kernel; a
+        // predicated FADD runs on the FMA pipe (same for dg above and U / L below)
+        float newD = 0.0f, newI = 0.0f;
+        if (pD) asm volatile("add.rn.f32 %0, %1, 0f3F800000;" : "=f"(newD) : "f"(st.lRunF));
+        if (pI) asm volatile("add.rn.f32 %0, %1, 0f3F800000;" : "=f"(newI) : "f"(upRunF));
+        const float runF = __fadd_rn(newD, newI);
+        const float pen = fminf(sc.ext_min, __fadd_rn(sc.gap_ext, __fmul_rn(runF, sc.decay)));
+        // e = (S == 0) ? 0 : S + pen  as one exact fused op: S + pen * [S != 0]
+        float nz;
+        asm("set.ne.f32.f32 %0, %1, 0f00000000;" : "=f"(nz) : "f"(S));
+        U = __fadd_rn(S, sc.open_read);
+        L = __fadd_rn(S, sc.open_ref);
+        if (pI) asm volatile("fma.rn.f32 %0, %1, %2, %3;" : "=f"(U) : "f"(pen), "f"(nz), "f"(S));
+        if (pD) asm volatile("fma.rn.f32 %0, %1, %2, %3;" : "=f"(L) : "f"(pen), "f"(nz), "f"(S));
+        st.oP = __float_as_uint(newI);
+        st.lRunF = newD;
+        st.lIsD = pD;
+      }
+      st.oS = S;
+      st.oU = U;
+      st.oC = r;
+      st.lL = L;
+      if (S > st.kS) {  // strict: first maximum in row-major order (:1165-1170)
+        // S + 0 == S bit for bit (S >= +0); as predicated FMA-pipe instructions instead of two selects
+        asm volatile("add.rn.f32 %0, %1, 0f00000000;" : "=f"(st.kS) : "f"(S));
+        asm volatile("mad.lo.s32 %0, %1, 1, 0;" : "=r"(st.kStep) : "r"(s));
+      }
+      dw = __funnelshift_r(dw, code, 2);
+#if FILL_LANE0_LDS
+      if (is31) iop[1] = make_uint4(__float_as_uint(st.oS), __float_as_uint(st.oU), st.oP, st.oC);
+#else
+      if (is31) {
+        // the record is exactly the four shuffle sources (w is rewritten when the chunk is staged)
+        iop[1] = make_uint4(__float_as_uint(st.oS), __float_as_uint(st.oU), st.oP, st.oC);
+        const uint4 t = iop[2];
+        st.oS = __uint_as_float(t.x);
+        st.oU = __uint_as_float(t.y);
+        st.oP = t.z;
+        st.oC = t.w;
+      }
+#endif
+      iop += 2;
+      if (!ALL_ACTIVE || RAW) ++st.rel;  // the RAW kernel needs the column for its tail rule
+    }
+  }
+  if (ALL_ACTIVE && !RAW) st.rel += 16;
+  // a lane whose 16 steps all lie outside its row has nothing the traceback will ever read: the block's
+  // leading and trailing wavefront stays out of HBM (whole 32-byte sectors, the idle lanes are neighbours)
+  if (ALL_ACTIVE || (st.rel > 0 && st.rel - 16 < (int)rlen)) dwp[(size_t)g * 32] = dw;
+}
+
 // NW = warps that pipeline ONE problem (1: every warp of the CTA has its own problem; otherwise the whole
 // CTA is the team: 4 warps for ordinary corridors, FILL_BIG_TEAM warps for the few huge matrices of a batch
 // -- a 10^8-cell realignment matrix would otherwise keep one 4-warp team busy long after the rest of the
@@ -285,26 +442,26 @@ convex_fill_kernel(const FillParams p) {
       }
       uint32_t* __restrict__ dwp = p.dir + word_off + lane;
 
-      int rel = base - lane - xlo;  // x - xlo at step 0; inside the corridor iff (unsigned)rel < rlen
       const int t0rel = (int)rlen > 12 ? (int)rlen - 12 : 0;  // tail start max(x0, xMax-12) - xlo (:1179)
 
-      // What this lane hands down / keeps for its right neighbour. EMPTY = {0, 0, STOP}.
-      // oP: scalar kernel = the I-run length as a float (0 unless the cell is an insertion);
-      //     RAW kernel    = indelRun (low 16 bits) | direction << 16.
-      float oS = 0.0f, oU = sc.open_read;
-      uint32_t oP = empty_pack, oC = 0u;
-      float dS = 0.0f;         // score of (x-1, y-1)
-      float lL = sc.open_ref;  // left_cell contribution of (x-1, y)
-      float lRunF = 0.0f;      // scalar kernel: D-run length of (x-1, y), 0 unless it is a deletion
-      bool lIsD = false;
-      int lRun = 0;            // RAW kernel: raw indelRun / direction of (x-1, y)
-      uint32_t lDir = DIR_STOP;
-      float kS = bestS;
-      int kStep = -1;
+      LaneState st;
+      st.rel = base - lane - xlo;  // x - xlo at step 0
+      st.oS = 0.0f;
+      st.oU = sc.open_read;
+      st.oP = empty_pack;
+      st.oC = 0u;
+      st.dS = 0.0f;
+      st.lL = sc.open_ref;
+      st.lRunF = 0.0f;
+      st.lIsD = false;
+      st.lRun = 0;
+      st.lDir = DIR_STOP;
+      st.kS = bestS;
+      st.kStep = -1;
 
       // stage chunk 0 (+ the diagonal neighbour of lane 0's first cell)
       wait_for(base + CHUNK);
-      if (is0) dS = __uint_as_float(strip_rec(base - 1).x);
+      if (is0) st.dS = __uint_as_float(strip_rec(base - 1).x);
       uint4 pa = EMPTY, pb = EMPTY;
       uint32_t ra = 0, rb = 0;
       {
@@ -328,10 +485,10 @@ convex_fill_kernel(const FillParams p) {
 #if !FILL_LANE0_LDS
         if (is31) {  // lane 31's shuffle sources carry the strip record lane 0 needs next
           const uint4 t = io_s[0];
-          oS = __uint_as_float(t.x);
-          oU = __uint_as_float(t.y);
-          oP = t.z;
-          oC = t.w;
+          st.oS = __uint_as_float(t.x);
+          st.oU = __uint_as_float(t.y);
+          st.oP = t.z;
+          st.oC = t.w;
         }
 #endif
         if (c + 1 < nchunks) {  // fetch the next chunk while this one is computed
@@ -347,140 +504,10 @@ convex_fill_kernel(const FillParams p) {
           }
         }
         const int g_end = min(ngroups, (c + 1) * GPC);
-        // A 16-step group in which every lane stays inside its corridor row needs no masking at all
-        // (the common case away from the block's leading and trailing wavefront).
-        auto do_group = [&](auto all_active_tag, int g) {
-          constexpr bool ALL_ACTIVE = decltype(all_active_tag)::value;
-          uint4* iop = io_s + ((g % GPC) << 5);  // [0] lane 0's input of this step, [1] lane 31's output
-          uint32_t dw = 0;
-          {
-#pragma unroll 2  // 2 keeps the per-step predicates in registers; 4 makes ptxas spill them to a bit mask
-            for (int k = 0; k < 16; ++k) {
-              const int s = (g << 4) + k;
-              uint4 v;
-#if FILL_LANE0_LDS
-              // lanes 1..31 take their upper neighbour's cell from lane t-1, lane 0 from the staged strip record
-              v.x = __float_as_uint(__shfl_up_sync(FULL, oS, 1));
-              v.y = __float_as_uint(__shfl_up_sync(FULL, oU, 1));
-              v.z = __shfl_up_sync(FULL, oP, 1);
-              v.w = __shfl_up_sync(FULL, oC, 1);
-              if (is0) v = iop[0];
-#else
-              v.x = __float_as_uint(__shfl_sync(FULL, oS, src_lane));
-              v.y = __float_as_uint(__shfl_sync(FULL, oU, src_lane));
-              v.z = __shfl_sync(FULL, oP, src_lane);
-              v.w = __shfl_sync(FULL, oC, src_lane);
-#endif
-              const float nS = __uint_as_float(v.x), nU = __uint_as_float(v.y);
-              const uint32_t r = v.w;
-              const bool act = ALL_ACTIVE ? true : ((unsigned)rel < rlen);
-              float dg = __fadd_rn(dS, sc.mis);
-              if (r == q) dg = __fadd_rn(dS, sc.mat);
-              dS = nS;
-              // Outside the corridor the cell must degenerate to {0, 0, STOP}: a NaN maximum makes every
-              // equality below false, and fmaxf(NaN, 0) = 0 gives the score.
-              const float m0 = fmaxf(fmaxf(fmaxf(lL, 0.0f), dg), nU);
-              const float m = (ALL_ACTIVE || act) ? m0 : __int_as_float(0x7fffffff);
-              const bool eL = (m == lL), eU = (m == nU), eG = (m == dg);
-              const float S = ALL_ACTIVE ? m : fmaxf(m, 0.0f);  // STOP implies m == 0
-              uint32_t code;
-              float U, L;
-              if (RAW) {
-                const uint32_t nP = v.z;
-                const int upRaw = (int)(short)(nP & 0xffffu);
-                const uint32_t upDir = (nP >> 16) & 3u;
-                const bool rawHere = rel < t0rel;
-                const int upRun = (rawHere || upDir == DIR_I) ? upRaw : 0;
-                const int leftRun = (rawHere || lDir == DIR_D) ? lRun : 0;
-                // priority (:1232-1267): continue D, continue I, diagonal, open D, open I, STOP
-                const bool dc = eL && (leftRun > 0);
-                const bool ic = !dc && eU && (upRun > 0);
-                const bool gg = !dc && !ic && eG;
-                const bool resolved = dc || ic || gg;
-                const bool isD = dc || (!resolved && eL);
-                const bool isI = ic || (!resolved && !eL && eU);
-                int run = dc ? leftRun : (ic ? upRun : 0);
-                run = (isD || isI) ? run + 1 : 0;
-                run = (int)(short)run;  // MatrixElement::indelRun is a short
-                code = gg ? DIR_DIAG : (isI ? DIR_I : (isD ? DIR_D : DIR_STOP));
-                // what the neighbours will see: S + min(ext_min, gap_ext + run*decay), 0 if S == 0 (:666-676)
-                const float pen = fminf(sc.ext_min, __fadd_rn(sc.gap_ext, __fmul_rn((float)run, sc.decay)));
-                float e = __fadd_rn(S, pen);
-                if (S == 0.0f) e = 0.0f;
-                U = isI ? e : __fadd_rn(S, sc.open_read);
-                L = isD ? e : __fadd_rn(S, sc.open_ref);
-                oP = (code << 16) | ((uint32_t)run & 0xffffu);
-                lRun = run;
-                lDir = code;
-              } else {
-                // Same priority chain as a 3-input predicate network (verified exhaustively):
-                //   D  <=>  eL && (lr || !((eU && ur) || eG))
-                //   I  <=>  !D && eU && (ur || !eG)
-                // with run lengths kept as floats (exact below 2^24; rows are < 32768 wide here).
-                const float upRunF = __uint_as_float(v.z);
-                const bool lr = lIsD, ur = upRunF > 0.0f;  // the left cell's run is > 0 iff it is a deletion
-                const bool X = (eU & ur) | eG;  // bitwise on purpose: straight PLOP3s, no short-circuit
-                const bool pD = eL & (lr | !X);
-                const bool pI = (!pD) & eU & (ur | !eG);
-                code = eG ? DIR_DIAG : DIR_STOP;
-                if (pI) asm volatile("mad.lo.u32 %0, %1, 0, 1;" : "=r"(code) : "r"(code));
-                if (pD) asm volatile("mad.lo.u32 %0, %1, 0, 2;" : "=r"(code) : "r"(code));
-                // at most one of the two run counters is alive after this cell
-                // "zero, then an addition under the predicate" instead of add + select: the selects, compares and
-                // min/max of this loop all go through the half-rate ALU pipe, which is what binds the kernel; a
-                // predicated FADD runs on the FMA pipe (same for dg above and U / L below)
-                float newD = 0.0f, newI = 0.0f;
-                if (pD) asm volatile("add.rn.f32 %0, %1, 0f3F800000;" : "=f"(newD) : "f"(lRunF));
-                if (pI) asm volatile("add.rn.f32 %0, %1, 0f3F800000;" : "=f"(newI) : "f"(upRunF));
-                const float runF = __fadd_rn(newD, newI);
-                const float pen = fminf(sc.ext_min, __fadd_rn(sc.gap_ext, __fmul_rn(runF, sc.decay)));
-                // e = (S == 0) ? 0 : S + pen  as one exact fused op: S + pen * [S != 0]
-                float nz;
-                asm("set.ne.f32.f32 %0, %1, 0f00000000;" : "=f"(nz) : "f"(S));
-                U = __fadd_rn(S, sc.open_read);
-                L = __fadd_rn(S, sc.open_ref);
-                if (pI) asm volatile("fma.rn.f32 %0, %1, %2, %3;" : "=f"(U) : "f"(pen), "f"(nz), "f"(S));
-                if (pD) asm volatile("fma.rn.f32 %0, %1, %2, %3;" : "=f"(L) : "f"(pen), "f"(nz), "f"(S));
-                oP = __float_as_uint(newI);
-                lRunF = newD;
-                lIsD = pD;
-              }
-              oS = S;
-              oU = U;
-              oC = r;
-              lL = L;
-              if (S > kS) {  // strict: first maximum in row-major order (:1165-1170)
-                // S + 0 == S bit for bit (S >= +0); as predicated FMA-pipe instructions instead of two selects
-                asm volatile("add.rn.f32 %0, %1, 0f00000000;" : "=f"(kS) : "f"(S));
-                asm volatile("mad.lo.s32 %0, %1, 1, 0;" : "=r"(kStep) : "r"(s));
-              }
-              dw = __funnelshift_r(dw, code, 2);
-#if FILL_LANE0_LDS
-              if (is31) iop[1] = make_uint4(__float_as_uint(oS), __float_as_uint(oU), oP, oC);
-#else
-              if (is31) {
-                // the record is exactly the four shuffle sources (w is rewritten when the chunk is staged)
-                iop[1] = make_uint4(__float_as_uint(oS), __float_as_uint(oU), oP, oC);
-                const uint4 t = iop[2];
-                oS = __uint_as_float(t.x);
-                oU = __uint_as_float(t.y);
-                oP = t.z;
-                oC = t.w;
-              }
-#endif
-              iop += 2;
-              if (!ALL_ACTIVE || RAW) ++rel;  // the RAW kernel needs the column for its tail rule
-            }
-          }
-          if (ALL_ACTIVE && !RAW) rel += 16;
-          // a lane whose 16 steps all lie outside its row has nothing the traceback will ever read: the block's
-          // leading and trailing wavefront stays out of HBM (whole 32-byte sectors, the idle lanes are neighbours)
-          if (ALL_ACTIVE || (rel > 0 && rel - 16 < (int)rlen)) dwp[(size_t)g * 32] = dw;
-        };
         for (int g = c * GPC; g < g_end; ++g) {
-          const bool all_active = __all_sync(FULL, rel >= 0 && rel + 15 < (int)rlen);
-          if (all_active) do_group(std::true_type{}, g);
-          else do_group(std::false_type{}, g);
+          const bool all_active = __all_sync(FULL, st.rel >= 0 && st.rel + 15 < (int)rlen);
+          if (all_active) fill_group<RAW, true, GPC>(st, sc, io_s, dwp, g, rlen, q, t0rel, is0, is31, src_lane);
+          else fill_group<RAW, false, GPC>(st, sc, io_s, dwp, g, rlen, q, t0rel, is0, is31, src_lane);
         }
         __syncwarp();
         // flush lane 31's records of this chunk: columns [base - 31 + CHUNK*c, ...)
@@ -498,10 +525,10 @@ convex_fill_kernel(const FillParams p) {
         __syncwarp();
       }
 
-      if (kStep >= 0) {
-        bestS = kS;
+      if (st.kStep >= 0) {
+        bestS = st.kS;
         bestY = y;
-        bestX = base + kStep - lane;
+        bestX = base + st.kStep - lane;
       }
       if (NW == 1) {
         wlo = base - 31;
@@ -570,9 +597,442 @@ convex_fill_kernel(const FillParams p) {
   }
 }
 
+// ---- ramp-free schedule -------------------------------------------------------------------------------------------
+// The kernel above runs a block's 32 rows in lockstep from the block's first column to its last: lane t of a block
+// whose corridor advances ~1 column per row idles ~2t steps before its row starts and ~2(31-t) steps after it ends,
+// W + ~62 steps for W useful ones. Here every lane moves on to its row of the warp's next block as soon as its own
+// part of the current one is done, so a warp step evaluates ~32 cells wherever the block boundary is. One warp per
+// problem: teams of this schedule wait on each other's strip hand-off (a team of NW warps needs corridors wider than
+// NW * (32 * (1 + slope) + hand-off latency) to run without stalls) and measured slower than one warp per problem.
+//
+// Within a block nothing changes: lane t evaluates column x of row 32b+t at warp step O_b + t + x, so every shuffle
+// dependency is the lockstep one. Lane t sweeps the columns [A, E) of block b, A = min(xlo_t, xlo_t+1) - 1,
+// E = max(xhi_t, xhi_t+1): that covers its row, the up / diagonal neighbours lane t+1 reads from it, and one
+// out-of-corridor step first, which resets its left neighbour state. Lane 31's range reaches the block's rightmost
+// column (the strip window of the next block). A lane enters block b at a 16-step group boundary (the switch costs
+// nothing inside a group, and a direction word holds one row), the last such boundary at or before step O_b + t + A.
+// O_b is the least origin that satisfies, for every lane:
+//   - its entry comes after the end of its previous range (no overlap within a lane);
+//   - its entry comes at least one chunk after the chunk in which the last lane entered the previous block: the
+//     warp keeps two blocks' descriptions (shared memory) and places the next one at a chunk boundary;
+//   - O_b >= O_{b-1} + RING: lane 31's record of column x, flushed at the end of its chunk, must be in the strip when
+//     lane 0 of the next block stages x two chunks ahead (31 + 2 chunks).
+// The reference byte of a column travels down the lanes with the cell values. A lane outside its row no longer gets a
+// valid one from above (the lane two rows up may have moved on), so there it loads the byte itself: every lane that
+// is inside its row then receives it from a lane that is in the same block.
+// Direction words: the warp's 16-step groups are numbered from its first step, and each block's BlockRec maps its
+// cells into them (base = 16 * first group - O_b): readers see the lockstep layout.
+constexpr int RF_NONE = INT_MIN;  // no entry: the lane has no columns in that block
+
+struct RfFrame {
+  int blk;        // -1: none
+  int O;          // lane t evaluates column x of row 32 * blk + t at warp step O + t + x
+  int wlo, whi;   // strip columns lane 31 of block blk-1 wrote (what lane 0 reads; everything else is EMPTY)
+  int a31, e31;   // lane 31's columns [a31, e31)
+  int sw0, sw31;  // entry steps of lanes 0 and 31 (RF_NONE: none)
+  int swmax;      // entry step of the last lane (no entries: the earliest allowed one - 1)
+};
+
+struct RfWarp {
+  unsigned long long word_off;  // the warp's direction words: group g of its steps at word_off + 32 g
+  int G;                        // groups of 16 steps the warp runs for its problem
+  int next_b, R, O_last;        // the block to place next, its earliest entry, the last placed origin
+  int firstX, firstY;           // first visited cell
+};
+
+// Lane t's columns [A, E) of a block (A = INT_MAX: none), from its row and the row below.
+__device__ __forceinline__ void rf_cols(int xlo, int xhi, unsigned rlen, int lane, int& A, int& E) {
+  const int a = rlen ? xlo : INT_MAX;
+  const int e = rlen ? xhi : INT_MIN;
+  int a1 = __shfl_down_sync(FULL, a, 1), e1 = __shfl_down_sync(FULL, e, 1);
+  const int emax = __reduce_max_sync(FULL, e);
+  if (lane == 31) {
+    a1 = INT_MAX;
+    e1 = emax;
+  }
+  const int amin = min(a, a1);
+  A = amin == INT_MAX ? INT_MAX : amin - 1;
+  E = max(e, e1);
+}
+
+// Origin and entry steps of block b. L: end of the lane's previous range (RF_NONE: none); R: earliest entry;
+// O_min: the hand-off bound.
+__device__ __forceinline__ void rf_place(const CorridorView& cv, int b, int lane, int H, int ref_len, int L, int R,
+                                         int O_min, int& xlo, unsigned& rlen, int& A, int& E, int& O, int& sw) {
+  int off, len, xhi;
+  load_corridor_rows(cv, b, lane, H, off, len);
+  row_span(off, len, ref_len, xlo, xhi, rlen);
+  rf_cols(xlo, xhi, rlen, lane, A, E);
+  const int from = max(L, R);
+  const int need = A == INT_MAX ? INT_MIN : ((from + 15) & ~15) - lane - A;
+  O = max(O_min, __reduce_max_sync(FULL, need));
+  sw = A == INT_MAX ? RF_NONE : ((O + lane + A) & ~15);
+}
+
+constexpr int RF_CHUNK = 64;                  // steps staged through shared memory at a time
+constexpr int RF_RING = 32 + 2 * RF_CHUNK;    // hand-off spacing of consecutive origins
+
+// the earliest entry into the block after one whose last lane enters at step swmax
+__device__ __forceinline__ int rf_next_entry(int swmax) { return ((swmax + RF_CHUNK) / RF_CHUNK + 1) * RF_CHUNK; }
+
+template <bool RAW, bool PERSIST>
+__global__ void __launch_bounds__(FILL_WARPS_PER_CTA * 32, FILL_CTAS_PER_SM)
+convex_fill_rf_kernel(const FillParams p) {
+  constexpr int WARPS = FILL_WARPS_PER_CTA;
+  constexpr int CHUNK = RF_CHUNK;
+  constexpr int GPC = CHUNK / 16;
+  __shared__ uint4 s_io[WARPS][2 * (CHUNK + 1)];
+  __shared__ int s_slot;
+  __shared__ RfFrame s_f0[WARPS], s_f31[WARPS], s_nx[WARPS];  // the blocks lanes 0 / 31 are in, the next block
+  __shared__ int4 s_nrow[WARPS][32];     // the lane's row of the next block: {rel at entry, rlen, q}
+  __shared__ int4 s_cur[WARPS][32];      // {O, y} of the lane's current row, L = end of its last range, its cells
+  __shared__ float4 s_bestl[WARPS][32];  // the lane's best cell of its finished rows {S, x, y}
+  __shared__ RfWarp s_w[WARPS];
+  const int lane = threadIdx.x & 31;
+  const int wib = threadIdx.x >> 5;
+  if (!PERSIST) {  // as in convex_fill_kernel; the slot is given back from s_slot (no registers held meanwhile)
+    if (threadIdx.x == 0) {
+      unsigned smid;
+      asm("mov.u32 %0, %%smid;" : "=r"(smid));
+      int got = -1;
+      for (;;) {
+        for (int b = 0; b < p.sm_slot_count && got < 0; ++b)
+          if (!(atomicOr(p.sm_slots + smid, 1u << b) & (1u << b))) got = b;
+        if (got >= 0) break;
+        __nanosleep(2000);
+      }
+      s_slot = (int)smid * FILL_SM_SLOTS + got;
+    }
+    __syncthreads();
+  }
+  const int cta_slot = PERSIST ? (int)blockIdx.x : s_slot;
+  uint4* const io_s = s_io[wib];
+  uint4* const strip = reinterpret_cast<uint4*>(p.bnd) + (size_t)(cta_slot * WARPS + wib) * p.bnd_stride + STRIP_PAD;
+  const Scoring sc = p.sc;
+  const uint32_t empty_pack = RAW ? (DIR_STOP << 16) : 0u;
+  const uint4 EMPTY = make_uint4(0u, __float_as_uint(sc.open_read), empty_pack, 0u);
+  const bool is0 = lane == 0, is31 = lane == 31;
+  const int src_lane = (lane + 31) & 31;
+  RfWarp& ws = s_w[wib];
+
+  for (int taken = 0; PERSIST || taken < p.problems_per_cta; ++taken) {
+    int w = 0;
+    if (is0) w = atomicAdd(p.work_counter, 1);
+    w = __shfl_sync(FULL, w, 0) + p.first;
+    if (w >= p.last) break;
+    const int ai = p.order[w];
+    // The descriptor and the corridor view are re-read where they are needed (block boundaries) instead of being
+    // kept in registers across the cell loop; likewise the warp's bookkeeping lives in shared memory.
+    auto corridor = [&]() {
+      CorridorView cv;
+      cv.bind(p.c_off, p.c_len, p.c_blkbase, p.c_delta, p.desc[ai]);
+      return cv;
+    };
+    const uint8_t* __restrict__ ref = p.seq + p.desc[ai].ref_off;
+    const unsigned ref_len = (unsigned)p.desc[ai].ref_len;
+    int status = ST_OK;
+
+    // Pass 1: the warp's schedule (the same placements as pass 2 makes) -> its number of steps.
+    {
+      const CorridorView cv = corridor();
+      const int H = p.desc[ai].height, nblk = (H + 31) >> 5;
+      int L = RF_NONE, R = 0, O_last = RF_NONE;
+      for (int b = 0; b < nblk; ++b) {
+        int xlo, A, E, O, sw;
+        unsigned rlen;
+        rf_place(cv, b, lane, H, (int)ref_len, L, R, O_last == RF_NONE ? INT_MIN : O_last + RF_RING, xlo, rlen, A, E,
+                 O, sw);
+        if (__any_sync(FULL, sw != RF_NONE)) O_last = O;
+        if (sw != RF_NONE) L = O + lane + E;
+        R = rf_next_entry(__reduce_max_sync(FULL, sw != RF_NONE ? sw : R - 1));
+      }
+      const int T = max(0, __reduce_max_sync(FULL, L));
+      const int G = (T + 15) >> 4;
+      unsigned long long wo = 0;
+      if (is0) wo = atomicAdd(p.dir_alloc, (unsigned long long)G * 32ull);
+      wo = __shfl_sync(FULL, wo, 0);
+      if (wo + (unsigned long long)G * 32ull > p.dir_capacity) status = ST_DIR_OVERFLOW;
+      if (is0) {
+        ws.word_off = wo;
+        ws.G = G;
+        ws.next_b = 0;
+        ws.R = 0;
+        ws.O_last = RF_NONE;
+        ws.firstX = 0;
+        ws.firstY = -1;
+        RfFrame none;
+        none.blk = -1;
+        none.O = none.wlo = none.whi = none.a31 = none.e31 = 0;
+        none.sw0 = none.sw31 = RF_NONE;
+        none.swmax = 0;
+        s_f0[wib] = none;
+        s_f31[wib] = none;
+        s_nx[wib] = none;
+      }
+      s_cur[wib][lane] = make_int4(0, 0, RF_NONE, 0);
+      s_bestl[wib][lane] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+      __syncwarp();
+    }
+    uint32_t* __restrict__ dwp = p.dir + ws.word_off + lane;
+
+    // Pass 2.
+    LaneState st;
+    st.rel = 0;
+    st.oS = 0.0f;
+    st.oU = sc.open_read;
+    st.oP = empty_pack;
+    st.oC = 0u;
+    st.dS = 0.0f;
+    st.lL = sc.open_ref;
+    st.lRunF = 0.0f;
+    st.lIsD = false;
+    st.lRun = 0;
+    st.lDir = DIR_STOP;
+    st.kS = 0.0f;
+    st.kStep = -1;
+    unsigned rlen = 0;  // before its first row a lane is outside every corridor
+    uint32_t q = 0x100u;
+    int t0rel = 0;
+    int sw = RF_NONE;   // step at which this lane enters the next block
+
+    // next block -> s_nx / s_nrow / sw, its BlockRec, the lane's cells and the warp's first visited cell
+    auto place = [&]() {
+      const CorridorView cv = corridor();
+      const AlnDesc* dp = p.desc + ai;
+      const int H = dp->height;
+      const int b = ws.next_b, R = ws.R, O_last = ws.O_last;
+      int4 me = s_cur[wib][lane];
+      int nxlo, A, E, O, swl;
+      unsigned rl;
+      rf_place(cv, b, lane, H, (int)ref_len, me.z, R, O_last == RF_NONE ? INT_MIN : O_last + RF_RING, nxlo, rl, A, E,
+               O, swl);
+      const bool any = __any_sync(FULL, swl != RF_NONE);
+      if (swl != RF_NONE) me.z = O + lane + E;
+      me.w += (int)rl;  // cells of this lane's rows (< 2^32 for every problem the ordinary launches get)
+      const int swmax = __reduce_max_sync(FULL, swl != RF_NONE ? swl : R - 1);
+      const int y = (b << 5) + lane;
+      const int4 nrow = make_int4(swl - (O + lane + nxlo), (int)rl, y < H ? (int)p.seq[dp->qry_off + y] : 0x100, 0);
+      const unsigned hit = __ballot_sync(FULL, rl != 0);
+      const int fx = hit ? __shfl_sync(FULL, nxlo, __ffs(hit) - 1) : 0;
+      // lane 31's columns of block b-1: what lane 0 of block b reads from the strip
+      int wlo = 0, whi = 0;
+      if (b > 0) {
+        int pxlo, pxhi, poff, plen, pA, pE;
+        unsigned prl;
+        load_corridor_rows(cv, b - 1, lane, H, poff, plen);
+        row_span(poff, plen, (int)ref_len, pxlo, pxhi, prl);
+        rf_cols(pxlo, pxhi, prl, lane, pA, pE);
+        pA = __shfl_sync(FULL, pA, 31);
+        pE = __shfl_sync(FULL, pE, 31);
+        if (pA != INT_MAX) {
+          wlo = pA;
+          whi = pE;
+        }
+      }
+      const int g0 = __reduce_min_sync(FULL, swl != RF_NONE ? swl : INT_MAX);
+      const int end = __reduce_max_sync(FULL, swl != RF_NONE ? O + lane + E : INT_MIN);
+      const int a31 = __shfl_sync(FULL, A, 31), e31 = __shfl_sync(FULL, E, 31);
+      const int sw0 = __shfl_sync(FULL, swl, 0), sw31 = __shfl_sync(FULL, swl, 31);
+      s_cur[wib][lane] = me;
+      s_nrow[wib][lane] = nrow;
+      sw = swl;
+      __syncwarp();
+      if (is0) {
+        BlockRec br;
+        br.word_off = ws.word_off + (any ? (unsigned long long)(g0 >> 4) * 32ull : 0ull);
+        br.base = any ? g0 - O : 0;
+        br.nsteps = any ? end - g0 : 0;
+        p.blocks[dp->blk_off + b] = br;
+        RfFrame f;
+        f.blk = b;
+        f.O = O;
+        f.wlo = wlo;
+        f.whi = whi;
+        f.a31 = a31;
+        f.e31 = e31;
+        f.sw0 = sw0;
+        f.sw31 = sw31;
+        f.swmax = swmax;
+        s_nx[wib] = f;
+        ws.next_b = b + 1;
+        ws.R = rf_next_entry(swmax);
+        if (any) ws.O_last = O;
+        if (hit && ws.firstY < 0) {
+          ws.firstY = (b << 5) + __ffs(hit) - 1;
+          ws.firstX = fx;
+        }
+      }
+      __syncwarp();
+    };
+    // the strip records and reference bytes lane 0 consumes at steps [kk * CHUNK, (kk + 1) * CHUNK): record j is
+    // the record of lane 0's column at step kk * CHUNK + j in the block lane 0 is in at that step
+    uint4 pa = EMPTY, pb = EMPTY;
+    auto stage = [&](int kk) {
+      const RfFrame* n = &s_nx[wib];
+      const RfFrame* f = &s_f0[wib];
+      const int nblk_ = n->blk, nsw0 = n->sw0, fblk = f->blk;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int sigma = kk * CHUNK + lane + 32 * h;
+        const bool in_n = nblk_ >= 0 && nsw0 != RF_NONE && sigma >= nsw0;
+        const RfFrame* fr = in_n ? n : f;
+        const int col = sigma - fr->O;
+        uint4 rec = EMPTY;
+        if (in_n || fblk >= 0) {
+          if (col >= fr->wlo && col < fr->whi) rec = ld_strip(strip + col);
+          rec.w = (unsigned)col < ref_len ? __ldg(ref + col) : 0u;  // the column's reference byte
+        }
+        if (h == 0) pa = rec;
+        else pb = rec;
+      }
+    };
+
+    const int nchunks = status == ST_OK ? (ws.G + GPC - 1) / GPC : 0;
+    if (nchunks > 0) {
+      place();
+      stage(0);
+    }
+    for (int c = 0; c < nchunks; ++c) {
+      // every lane has entered the next block: it becomes the current one, and the one after it is placed
+      for (;;) {
+        const RfFrame n = s_nx[wib];
+        if (n.blk < 0 || n.swmax >= c * CHUNK) break;
+        __syncwarp();
+        if (is0) {
+          if (n.sw0 != RF_NONE) s_f0[wib] = n;
+          if (n.sw31 != RF_NONE) s_f31[wib] = n;
+          s_nx[wib].blk = -1;
+        }
+        __syncwarp();
+        if (ws.next_b < ((p.desc[ai].height + 31) >> 5)) place();
+        else sw = RF_NONE;
+      }
+      io_s[2 * lane] = pa;
+      io_s[2 * (lane + 32)] = pb;
+      __syncwarp();
+#if !FILL_LANE0_LDS
+      if (is31) {
+        const uint4 t = io_s[0];
+        st.oS = __uint_as_float(t.x);
+        st.oU = __uint_as_float(t.y);
+        st.oP = t.z;
+        st.oC = t.w;
+      }
+#endif
+      if (c + 1 < nchunks) stage(c + 1);
+      const int g_end = min(ws.G, (c + 1) * GPC);
+      for (int g = c * GPC; g < g_end; ++g) {
+        if ((g << 4) == sw) {  // this lane enters its row of the next block
+          int4 me = s_cur[wib][lane];
+          if (st.kStep >= 0) {
+            s_bestl[wib][lane] = make_float4(st.kS, __int_as_float(st.kStep - me.x - lane), __int_as_float(me.y), 0.0f);
+            st.kStep = -1;
+          }
+          const int4 nr = s_nrow[wib][lane];
+          st.rel = nr.x;
+          rlen = (unsigned)nr.y;
+          q = (uint32_t)nr.z;
+          t0rel = nr.y > 12 ? nr.y - 12 : 0;
+          me.x = s_nx[wib].O;
+          me.y = (s_nx[wib].blk << 5) + lane;
+          s_cur[wib][lane] = me;
+          sw = RF_NONE;
+        }
+        const bool all_active = __all_sync(FULL, st.rel >= 0 && st.rel + 15 < (int)rlen);
+        if (all_active) {
+          fill_group<RAW, true, GPC>(st, sc, io_s, dwp, g, rlen, q, t0rel, is0, is31, src_lane);
+        } else {
+          // column of the lane at step s: s - (O + lane), O of the row it is in
+          fill_group<RAW, false, GPC, true>(st, sc, io_s, dwp, g, rlen, q, t0rel, is0, is31, src_lane, ref,
+                                             s_cur[wib][lane].x + lane, ref_len);
+        }
+      }
+      __syncwarp();
+      // flush lane 31's records of this chunk that lie in its columns of the block it was in
+      {
+        const RfFrame* n = &s_nx[wib];
+        const RfFrame* f = &s_f31[wib];
+        const int done = (g_end - c * GPC) << 4;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int j = lane + 32 * h;
+          const int sigma = c * CHUNK + j;
+          const bool in_n = n->blk >= 0 && n->sw31 != RF_NONE && sigma >= n->sw31;
+          const RfFrame* fr = in_n ? n : f;
+          const int x = sigma - fr->O - 31;
+          if (j < done && (in_n || f->blk >= 0) && x >= fr->a31 && x < fr->e31) st_strip(strip + x, io_s[2 * j + 1]);
+        }
+      }
+      __syncwarp();
+    }
+    const int4 me = s_cur[wib][lane];
+    const float4 bl = s_bestl[wib][lane];
+    float bestS = bl.x;
+    int bestX = __float_as_int(bl.y), bestY = __float_as_int(bl.z);
+    if (st.kStep >= 0) {
+      bestS = st.kS;
+      bestX = st.kStep - me.x - lane;
+      bestY = me.y;
+    }
+    unsigned long long cells = (unsigned)me.w;
+    // blocks the schedule never reached have no cells
+    if (is0 && status == ST_OK)
+      for (int b = ws.next_b; b < ((p.desc[ai].height + 31) >> 5); ++b) {
+        BlockRec br;
+        br.word_off = ws.word_off;
+        br.base = 0;
+        br.nsteps = 0;
+        p.blocks[p.desc[ai].blk_off + b] = br;
+      }
+
+    // first maximum in row-major order across lanes: larger score, then smaller y, then smaller x
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      const float s2 = __shfl_xor_sync(FULL, bestS, o);
+      const int y2 = __shfl_xor_sync(FULL, bestY, o);
+      const int x2 = __shfl_xor_sync(FULL, bestX, o);
+      const unsigned long long c2 = __shfl_xor_sync(FULL, cells, o);
+      const bool take = (s2 > bestS) || (s2 == bestS && (y2 < bestY || (y2 == bestY && x2 < bestX)));
+      if (take) {
+        bestS = s2;
+        bestY = y2;
+        bestX = x2;
+      }
+      cells += c2;
+    }
+    if (bestS == 0.0f) {  // no positive score anywhere: the first visited cell stands (or nothing was visited)
+      const bool any = ws.firstY >= 0;
+      bestS = any ? 0.0f : -1.0f;
+      bestX = any ? ws.firstX : 0;
+      bestY = any ? ws.firstY : 0;
+    }
+    if (is0) {
+      FillOut o;
+      o.best_score = bestS;
+      o.best_x = bestX;
+      o.best_y = bestY;
+      o.status = status;
+      o.cells = cells;
+      p.out[ai] = o;
+    }
+    __syncwarp();
+  }
+  if (!PERSIST) {
+    __syncthreads();
+    if (threadIdx.x == 0) atomicAnd(p.sm_slots + s_slot / FILL_SM_SLOTS, ~(1u << (s_slot % FILL_SM_SLOTS)));
+  }
+}
+
 }  // namespace
 
 namespace {
+template <bool RAW>
+void launch_fill_rf(const FillParams& p, int grid, cudaStream_t stream) {
+  const int threads = FILL_WARPS_PER_CTA * 32;
+  if (p.sm_slots) convex_fill_rf_kernel<RAW, false><<<grid, threads, 0, stream>>>(p);
+  else convex_fill_rf_kernel<RAW, true><<<grid, threads, 0, stream>>>(p);
+}
+
 template <bool RAW, int NW>
 void launch_fill(const FillParams& p, int grid, cudaStream_t stream) {
   const int threads = (NW == 1 ? FILL_WARPS_PER_CTA : NW) * 32;
@@ -582,8 +1042,11 @@ void launch_fill(const FillParams& p, int grid, cudaStream_t stream) {
 }  // namespace
 
 // p.sm_slots != nullptr selects the short-lived-CTA instantiation (one problem per warp / team, strips by SM slot)
-cudaError_t launch_convex_fill(const FillParams& p, bool raw, bool team, int grid, cudaStream_t stream) {
-  if (raw) {
+cudaError_t launch_convex_fill(const FillParams& p, bool raw, bool team, bool rampfree, int grid, cudaStream_t stream) {
+  if (rampfree) {
+    if (raw) launch_fill_rf<true>(p, grid, stream);
+    else launch_fill_rf<false>(p, grid, stream);
+  } else if (raw) {
     if (team) launch_fill<true, FILL_WARPS_PER_CTA>(p, grid, stream);
     else launch_fill<true, 1>(p, grid, stream);
   } else {
@@ -600,15 +1063,16 @@ cudaError_t launch_convex_fill_big(const FillParams& p, bool raw, int grid, cuda
   return cudaGetLastError();
 }
 
-int fill_max_ctas_per_sm(bool raw, bool team) {
+int fill_max_ctas_per_sm(bool raw, bool team, bool rampfree) {
   int n = 0;
   const int threads = FILL_WARPS_PER_CTA * 32;
-  if (raw) {
-    if (team) cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, convex_fill_kernel<true, FILL_WARPS_PER_CTA, true>, threads, 0);
-    else cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, convex_fill_kernel<true, 1, true>, threads, 0);
+  auto occ = [&](auto kernel) { cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, kernel, threads, 0); };
+  if (rampfree) {
+    raw ? occ(convex_fill_rf_kernel<true, true>) : occ(convex_fill_rf_kernel<false, true>);
+  } else if (raw) {
+    team ? occ(convex_fill_kernel<true, FILL_WARPS_PER_CTA, true>) : occ(convex_fill_kernel<true, 1, true>);
   } else {
-    if (team) cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, convex_fill_kernel<false, FILL_WARPS_PER_CTA, true>, threads, 0);
-    else cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, convex_fill_kernel<false, 1, true>, threads, 0);
+    team ? occ(convex_fill_kernel<false, FILL_WARPS_PER_CTA, true>) : occ(convex_fill_kernel<false, 1, true>);
   }
   return n;
 }

@@ -82,7 +82,7 @@ int convex_upload_spec(ngmlr_b200_ctx* ctx, const UploadSpec& sp) {
     tb_ints = tb_;
   }
   std::vector<unsigned long long> est(n);
-  std::vector<size_t> dirw(n);
+  std::vector<size_t> dirw(n), dirw_rf(n);
   std::vector<int> maxlen(n);
   std::vector<uint8_t> orderly(n);  // corridor never moves left and rows are never empty in the middle
   parallel_for(n, forms ? 256 : 16, [&](int i) {
@@ -167,28 +167,37 @@ int convex_upload_spec(ngmlr_b200_ctx* ctx, const UploadSpec& sp) {
     maxlen[i] = std::min(ml, rl);
     est[i] = sum;
     // direction arena estimate: per 32-row block, steps = row width + 31 (stagger) + corridor
-    // advance over the block; the exact figure is computed by the kernel (bump allocation) and an
+    // advance over the block; for the ramp-free kernel at least what its hand-off spacing costs a
+    // narrow corridor. The exact figure is computed by the kernel (bump allocation) and an
     // overflow triggers a re-run with a larger arena.
-    dirw[i] = 0;
+    dirw[i] = dirw_rf[i] = 0;
     if (ql > 0) {
       const long long adv_total = std::max<long long>(0, last_off - first_off);
       const long long adv = (adv_total * 32 + std::max(ql - 1, 1) - 1) / std::max(ql - 1, 1) + 2;
       const long long w = std::min<long long>(ml, (long long)rl);
-      const long long steps = w + 31 + adv;
+      const long long steps = w + 31 + adv, steps_rf = std::max<long long>(steps, RF_MIN_BLOCK_STEPS);
       dirw[i] = (size_t)(((size_t)ql + 31) / 32) * (size_t)((steps + 15) / 16 + 1) * 32;
+      dirw_rf[i] = (size_t)(((size_t)ql + 31) / 32) * (size_t)((steps_rf + 15) / 16 + 1) * 32;
     }
   });
   int max_len_all = 0;
-  size_t dir_words = 0, qry_total = 0, ref_total = 0;
+  size_t dir_words = 0, dir_words_rf = 0, qry_total = 0, ref_total = 0;
   ctx->max_ref_len = 0;
   ctx->wide_problems = 0;
   ctx->team_safe = true;
+  ctx->rf_wide = 0;
+  ctx->rf_fits = true;
   for (int i = 0; i < n; ++i) {
+    // The ramp-free kernel numbers the steps of a problem in an int: a block adds at most its column span
+    // (<= refLen + 1) plus the hand-off and placement slack (< 400 steps) -- keep the total below 2^30.
+    if ((((long long)qry_lens[i] + 31) / 32) * ((long long)ref_lens[i] + 400) >= (1ll << 30)) ctx->rf_fits = false;
     if (!orderly[i]) ctx->team_safe = false;
     if (maxlen[i] >= 352) ctx->wide_problems++;
+    if (maxlen[i] >= RF_MIN_WIDTH) ctx->rf_wide++;
     max_len_all = std::max(max_len_all, maxlen[i]);
     ctx->max_ref_len = std::max(ctx->max_ref_len, ref_lens[i]);
     dir_words += dirw[i];
+    dir_words_rf += dirw_rf[i];
     qry_total += (size_t)qry_lens[i];
     ref_total += (size_t)ref_lens[i];
     ctx->ext_qs[i] = ctx->h_desc.p[i].ext_qstart;
@@ -204,6 +213,8 @@ int convex_upload_spec(ngmlr_b200_ctx* ctx, const UploadSpec& sp) {
     n_big += big[i];
   }
   ctx->n_big = n_big;
+  ctx->rf_team = 0;
+  for (int i = 0; i < n; ++i) ctx->rf_team += !big[i] && est[i] >= ctx->rf_team_cells;
   std::iota(ctx->h_order.p, ctx->h_order.p + n, 0);
   std::stable_sort(ctx->h_order.p, ctx->h_order.p + n,
                    [&](int a, int b) { return big[a] != big[b] ? big[a] > big[b] : est[a] > est[b]; });
@@ -213,6 +224,7 @@ int convex_upload_spec(ngmlr_b200_ctx* ctx, const UploadSpec& sp) {
   ctx->tb_ints = tb_ints;
   ctx->max_len = max_len_all;
   ctx->dir_words_needed = dir_words + dir_words / 16 + 1024;
+  ctx->dir_words_rf = dir_words_rf + dir_words_rf / 16 + 1024;
   ctx->windows_mode = windows;
   ctx->parts_mode = parts;
   ctx->forms_mode = forms;
@@ -419,8 +431,16 @@ int ngmlr_b200_convex_run(ngmlr_b200_ctx* ctx) {
   bool team = ctx->wide_problems * 2 > n;
   if (ctx->force_team >= 0) team = ctx->force_team != 0;
   team = team && ctx->team_safe;
-  const int variant = (raw ? 1 : 0) | (team ? 2 : 0);
-  if (!ctx->ctas_per_sm[variant]) ctx->ctas_per_sm[variant] = std::max(1, fill_max_ctas_per_sm(raw, team));
+  // Ramp-free schedule (convex_fill.cu, one warp per problem) when most corridors are at least RF_MIN_WIDTH wide:
+  // narrower ones lose more to the schedule's boundary hand-off spacing than the ramp costs them. The largest
+  // problems still get 4-warp teams, in a launch of their own (below). NGMLR_B200_FILL_TEAM=1 selects the ramped
+  // teams for everything, NGMLR_B200_FILL_SCHEDULE=ramped the ramped kernels everywhere (DESIGN.md section 4.1).
+  // (fill_schedule 2, NGMLR_B200_FILL_SCHEDULE=rampfree-all: every batch, whatever its widths -- test / tuning hook)
+  const bool rampfree = ctx->fill_schedule >= 1 && ctx->force_team != 1 && ctx->rf_fits &&
+                        (ctx->fill_schedule == 2 || ctx->rf_wide * 2 > n);
+  if (rampfree) team = false;
+  const int variant = (raw ? 1 : 0) | (team ? 2 : 0) | (rampfree ? 4 : 0);
+  if (!ctx->ctas_per_sm[variant]) ctx->ctas_per_sm[variant] = std::max(1, fill_max_ctas_per_sm(raw, team, rampfree));
   int per_sm = std::min(ctx->ctas_per_sm[variant], team ? (int)FILL_TEAM_CTAS_PER_SM : (int)FILL_CTAS_PER_SM);
   if (ctx->fill_resident > 0) per_sm = std::min(per_sm, ctx->fill_resident);
   if (ctx->fill_ctas_cap > 0) per_sm = std::min(per_sm, ctx->fill_ctas_cap);
@@ -451,8 +471,13 @@ int ngmlr_b200_convex_run(ngmlr_b200_ctx* ctx) {
   // throughput: every problem gets an SM and a 16-warp team of its own.
   if (big_ok && n <= ctx->num_sms && ctx->small_batch_big_teams) n_big = n;
   const int big_grid = std::min(n_big, ctx->num_sms);
-  CU(ctx->d_bnd.reserve((warps + (size_t)big_grid) * bnd_stride));
-  size_t dir_words = std::max(ctx->dir_words_needed, (size_t)4096);
+  // ramp-free schedule: the largest problems (they lead the order after the big ones) go to a persistent launch of
+  // ramped 4-warp teams beside the one-warp launch, one CTA per SM at most
+  const int n_team = rampfree && ctx->team_safe && ctx->force_team != 0 ? std::min(ctx->rf_team, n - n_big) : 0;
+  const int team_grid = std::min(n_team, ctx->num_sms);
+  CU(ctx->d_bnd.reserve((warps + (size_t)big_grid + (size_t)team_grid) * bnd_stride));
+  size_t& words_needed = rampfree ? ctx->dir_words_rf : ctx->dir_words_needed;
+  size_t dir_words = std::max(words_needed, (size_t)4096);
   if (ctx->debug_arena_words >= 0) {  // force the overflow -> grow -> re-run path (tests)
     dir_words = (size_t)ctx->debug_arena_words;
     ctx->d_dir.release();
@@ -484,7 +509,7 @@ int ngmlr_b200_convex_run(ngmlr_b200_ctx* ctx) {
       fp.desc = ctx->d_desc.p;
       fp.order = ctx->d_order.p;
       fp.n = n;
-      fp.first = n_big;
+      fp.first = n_big + n_team;
       fp.last = n;
       fp.sm_slots = persistent ? nullptr : ctx->d_sm_slots.p;
       fp.sm_slot_count = std::min(per_sm, (int)FILL_SM_SLOTS);
@@ -529,18 +554,33 @@ int ngmlr_b200_convex_run(ngmlr_b200_ctx* ctx) {
         CU(launch_convex_fill_big(fb, raw, big_grid, ctx->stream2));
         CU(cudaEventRecord(ctx->ev_big, ctx->stream2));
       }
-      if (n - n_big > 0) {
-        const int g = persistent ? grid : std::max(1, team ? n - n_big : (n - n_big + FILL_WARPS_PER_CTA - 1) / FILL_WARPS_PER_CTA);
+      if (n_team > 0) {
+        FillParams ft = fp;
+        ft.first = n_big;
+        ft.last = n_big + n_team;
+        ft.work_counter = reinterpret_cast<int*>(ctx->d_counters.p + 7);
+        ft.sm_slots = nullptr;
+        ft.sm_slot_count = 0;
+        ft.problems_per_cta = 0;
+        ft.bnd = ctx->d_bnd.p + (warps + (size_t)big_grid) * bnd_stride;
+        CU(cudaStreamWaitEvent(ctx->stream3, ctx->ev[0], 0));
+        CU(launch_convex_fill(ft, raw, true, false, team_grid, ctx->stream3));
+        CU(cudaEventRecord(ctx->ev_team, ctx->stream3));
+      }
+      const int n_rest = n - n_big - n_team;
+      if (n_rest > 0) {
+        const int g = persistent ? grid : std::max(1, team ? n_rest : (n_rest + FILL_WARPS_PER_CTA - 1) / FILL_WARPS_PER_CTA);
         if (persistent || !ctx->stream_fill) {
-          CU(launch_convex_fill(fp, raw, team, g, st));
+          CU(launch_convex_fill(fp, raw, team, rampfree, g, st));
         } else {  // on the low-priority stream, between two events of the context's stream
           CU(cudaStreamWaitEvent(ctx->stream_fill, ctx->ev[0], 0));
-          CU(launch_convex_fill(fp, raw, team, g, ctx->stream_fill));
+          CU(launch_convex_fill(fp, raw, team, rampfree, g, ctx->stream_fill));
           CU(cudaEventRecord(ctx->ev_fill, ctx->stream_fill));
           CU(cudaStreamWaitEvent(st, ctx->ev_fill, 0));
         }
       }
       if (n_big > 0) CU(cudaStreamWaitEvent(st, ctx->ev_big, 0));
+      if (n_team > 0) CU(cudaStreamWaitEvent(st, ctx->ev_team, 0));
       CU(cudaEventRecord(ctx->ev[1], st));
       CU(launch_convex_traceback(tp, st));
       CU(cudaEventRecord(ctx->ev[2], st));
@@ -583,7 +623,7 @@ int ngmlr_b200_convex_run(ngmlr_b200_ctx* ctx) {
         // the counter under-reports after an overflow (warps stop allocating), so also double and
         // fall back to the host's estimate
         dir_words = std::max({(size_t)dir_used + (size_t)dir_used / 8 + 4096, (size_t)ctx->d_dir.cap * 2,
-                              ctx->dir_words_needed});
+                              words_needed});
         again = true;
       }
       if (runs_used > ctx->d_runs.cap) {
@@ -615,7 +655,8 @@ int ngmlr_b200_convex_run(ngmlr_b200_ctx* ctx) {
     if (!again) break;
     if (attempt == 23) return ctx->fail("convex_run: arena sizing did not converge");
   }
-  ctx->dir_words_needed = std::max(ctx->dir_words_needed, (size_t)ctx->dir_used);
+  words_needed = std::max(words_needed, (size_t)ctx->dir_used);
+  if (rampfree) ctx->rf_problems += (unsigned long long)(n - n_big - n_team);
   float ms = 0;
   cudaEventElapsedTime(&ms, ctx->ev[0], ctx->ev[1]);
   ctx->stats.fill_ms = ms;

@@ -20,11 +20,18 @@ constexpr int FILL_CTAS_PER_SM = FILL_CTAS_OVERRIDE;
 constexpr int FILL_SM_SLOTS = 8;   // boundary strips per SM for launches of short-lived CTAs (>= resident CTAs per SM)
 constexpr int FILL_BIG_TEAM = 16;  // warps that pipeline one huge matrix (one CTA per SM)
 
-// team = all FILL_WARPS_PER_CTA warps of a CTA pipeline one problem; otherwise one warp per problem
-cudaError_t launch_convex_fill(const FillParams& p, bool raw, bool team, int grid, cudaStream_t stream);
+constexpr int RF_MIN_WIDTH = 128;  // one-warp launches take the ramp-free schedule when most corridors are this wide
+constexpr int RF_MIN_BLOCK_STEPS = 224;  // steps per 32-row block the ramp-free schedule may spend on a narrow corridor
+// with the ramp-free schedule, problems of at least this many cells are filled by FILL_WARPS_PER_CTA-warp teams in a
+// launch of their own: one warp would still be busy with them long after the rest of the batch is done
+constexpr unsigned long long RF_TEAM_CELLS = 8ull << 20;
+
+// team = all FILL_WARPS_PER_CTA warps of a CTA pipeline one problem; otherwise one warp per problem.
+// rampfree: one warp per problem in the ramp-free row schedule (convex_fill.cu; `team` is ignored).
+cudaError_t launch_convex_fill(const FillParams& p, bool raw, bool team, bool rampfree, int grid, cudaStream_t stream);
 // the same kernel with a FILL_BIG_TEAM-warp team per problem, for the huge matrices of a batch
 cudaError_t launch_convex_fill_big(const FillParams& p, bool raw, int grid, cudaStream_t stream);
-int fill_max_ctas_per_sm(bool raw, bool team);
+int fill_max_ctas_per_sm(bool raw, bool team, bool rampfree);
 // %nsmid of the current device: every %smid is below it (SM ids need not be dense in 0 .. SM count - 1); -1 on error
 int fill_sm_id_bound();
 

@@ -184,6 +184,7 @@ struct ngmlr_b200_ctx {
   int sm_ids = 0;                   // %nsmid: size of the per-SM slot table of the short-lived fill CTAs
   cudaStream_t stream = nullptr;
   cudaStream_t stream2 = nullptr;   // the big-team fill launch runs beside the ordinary one
+  cudaStream_t stream3 = nullptr;   // ... and so does the team launch of the ramp-free schedule's largest problems
   cudaStream_t stream_fill = nullptr;  // lowest priority: the launch of short-lived fill CTAs
   cudaEvent_t ev_fill = nullptr;
   int small_batch_big_teams = 1;    // NGMLR_B200_SMALL_BATCH_BIG_TEAMS=0: batches of <= num_sms problems keep 4-warp teams
@@ -192,6 +193,7 @@ struct ngmlr_b200_ctx {
   bool sm_slots_zeroed = false;
   nb::DevBuf<unsigned int> d_sm_slots;
   cudaEvent_t ev_big = nullptr;
+  cudaEvent_t ev_team = nullptr;
   cudaEvent_t ev_sync = nullptr;    // cudaEventBlockingSync: waiting host threads sleep instead of spinning
   bool spin_sync = false;           // NGMLR_B200_SPIN_SYNC=1: cudaStreamSynchronize (lowest latency, one busy CPU per waiter)
   unsigned long long big_cells = 8ull << 20;  // a problem is "big" from this many cells ...
@@ -212,11 +214,17 @@ struct ngmlr_b200_ctx {
   int wide_problems = 0;  // problems whose corridor is >= 352 columns wide
   int force_team = -1;
   bool team_safe = true;  // every corridor of the batch is monotone with non-empty rows
+  int rf_wide = 0;        // problems whose corridor is >= RF_MIN_WIDTH columns wide
+  bool rf_fits = true;    // every problem's ramp-free step count fits the kernel's int step numbers
+  unsigned long long rf_problems = 0;  // problems filled by the ramp-free kernel since the context was created
+  int rf_team = 0;        // problems after the big ones with >= rf_team_cells cells (they lead the order)
+  unsigned long long rf_team_cells = nb::RF_TEAM_CELLS;  // NGMLR_B200_RF_TEAM_CELLS
+  int fill_schedule = 1;  // 1: ramp-free row schedule where it applies, 2: for every batch, 0: ramped (NGMLR_B200_FILL_SCHEDULE)
   int fill_ctas_cap = 0;  // 0 = full occupancy
   nb::PinBuf<unsigned long long> h_win;   // decode_windows: start | arena offset | (sequenceLength, span) pairs
   nb::DevBuf<unsigned long long> d_win;
   int64_t upload_d2h_bytes = 0;
-  int ctas_per_sm[4] = {0, 0, 0, 0};  // occupancy of the four fill-kernel variants
+  int ctas_per_sm[8] = {};  // occupancy of the eight fill-kernel variants (raw x team x ramp-free)
   long long debug_arena_words = -1;    // test hook: initial direction-arena size
   nb::PinBuf<uint8_t> h_seq;
   nb::PinBuf<int32_t> h_coff, h_clen, h_order, h_blkbase;
@@ -240,9 +248,11 @@ struct ngmlr_b200_ctx {
   nb::DevBuf<int32_t> d_scratch;
   nb::DevBuf<nb::TraceOut> d_trace;
   nb::DevBuf<int32_t> d_runs;
-  // [0] dir_alloc, [1] runs_alloc, [2] work counter (as int), [4] text_alloc, [5] peaks_alloc, [6] nm_alloc
+  // [0] dir_alloc, [1] runs_alloc, [2] work counter (as int), [3] big-team and [7] ramp-free team work counters,
+  // [4] text_alloc, [5] peaks_alloc, [6] nm_alloc
   nb::DevBuf<unsigned long long> d_counters;
   size_t dir_words_needed = 0;
+  size_t dir_words_rf = 0;  // the same for the ramp-free kernel
   bool ran = false;
   unsigned long long runs_used = 0, dir_used = 0;
   int fill_grid = 0;
