@@ -147,6 +147,36 @@ int ref_cs_init_save(const char* fasta) {
   return 0;
 }
 
+// Same as ref_cs_init / ref_cs_init_save (save != 0), at chosen values of ngmlr's options -k, --kmer-skip,
+// --bin-size, -s, --min-kmer-hits (not a command-line option; IConfig's default is 0), --subread-length and
+// --subread-corridor. They are set in the configuration before anything reads it. The reference caches several of
+// them in function-local statics and singletons on first use (GetBin / ResolveBin, CollectResultsStd, ScoreBuffer,
+// SequenceProvider), so one process can serve one option set only.
+int ref_cs_init_opts(const char* fasta, int k, int kmer_skip, int bin_size, float sensitivity, int min_kmer_hits,
+                     int read_part_length, int read_part_corridor, int save) {
+  IConfig* c = new IConfig();
+  c->referenceFile = strdup(fasta);
+  c->queryFile = strdup(fasta);
+  c->outputFile = strdup("/dev/null");
+  c->skipSave = save == 0;
+  c->progress = false;
+  c->kmerLength = k;
+  c->kmerSkip = kmer_skip;
+  c->binSize = bin_size;
+  c->sensitivity = sensitivity;
+  c->minKmerHits = min_kmer_hits;
+  c->readPartLength = read_part_length;
+  c->readPartCorridor = read_part_corridor;
+  _config = c;
+  _Log::Init(0, 0);
+  _log = &Log;
+  CS::Init();
+  SequenceProvider.Init();
+  g_table = new CompactPrefixTable();
+  g_probe = new CSProbe();
+  return 0;
+}
+
 unsigned long long ref_cs_concat_len() { return SequenceProvider.GetConcatRefLen(); }
 int ref_cs_ref_count() { return SequenceProvider.GetRefCount(); }
 // contig name as SAMWriter prints it ("%.*s" of GetRefName)

@@ -283,7 +283,8 @@ class CsReference:
     def available(cls):
         return os.path.exists(cls.PATH)
 
-    def __init__(self, fasta_path):
+    def __init__(self, fasta_path, options=None):
+        """options: one of cs_cases.OPTION_SETS (ngmlr's defaults when None)."""
         assert CsReference._inited in (None, fasta_path), "reference singletons already initialised"
         self.lib = C.CDLL(self.PATH)
         lib = self.lib
@@ -292,7 +293,12 @@ class CsReference:
         lib.ref_cs_ref_len.restype = C.c_ulonglong
         lib.ref_cs_index.restype = C.c_void_p
         if CsReference._inited is None:
-            lib.ref_cs_init(fasta_path.encode())
+            if options is None:
+                lib.ref_cs_init(fasta_path.encode())
+            else:
+                o = options
+                lib.ref_cs_init_opts(fasta_path.encode(), o["k"], o["skip"], o["bin"], C.c_float(o["s"]),
+                                     o["min_hits"], o["rpl"], o["corridor"], 0)
             CsReference._inited = fasta_path
 
     @property
@@ -307,7 +313,8 @@ class CsReference:
         rt = C.POINTER(C.c_uint)()
         ip = self.lib.ref_cs_index(C.byref(il), C.byref(rt), C.byref(rl), C.byref(uo), C.byref(uc))
         raw = np.ctypeslib.as_array(C.cast(ip, C.POINTER(C.c_uint8)), shape=(il.value * 5,)).reshape(-1, 5)
-        tab = raw[:, :4].copy().view(np.uint32).reshape(-1)
+        tab = np.empty(il.value, dtype=np.uint32)
+        tab.view(np.uint8).reshape(-1, 4)[:] = raw[:, :4]   # no intermediate copy: a 15-mer index has 4^15 + 1 rows
         rci = raw[:, 4].copy().view(np.int8)
         pos = np.ctypeslib.as_array(rt, shape=(rl.value + 1,))[:rl.value].copy()
         assert uo.value == 0 and uc.value == 1

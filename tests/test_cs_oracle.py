@@ -198,10 +198,11 @@ class _OracleBackend:
                 for t, r, o, l in zip(tasks, refs, offsets, lengths)]
 
 
-def _interval_tasks(contigs, enc):
+def _interval_tasks(contigs, enc, read_part_length=256):
     """Intervals as processLongReadLIS would hand them to computeAlignment: read part, reference span
-    (with some slack or some shortfall), 256-bp anchors (some reverse-coded), corridor estimate; plus
-    realign / short-read / full-matrix variants and corridors that are too narrow at first."""
+    (with some slack or some shortfall), anchors of read_part_length bases (some reverse-coded), corridor
+    estimate; plus realign / short-read / full-matrix variants and corridors that are too narrow at first."""
+    rpl = read_part_length
     from ngmlr_b200 import corridor, synth
     from ngmlr_b200.intervals import IntervalTask
     rng = np.random.default_rng(77)
@@ -222,17 +223,17 @@ def _interval_tasks(contigs, enc):
         on_stop = enc.ref_start[c] + s0 + L + int(rng.integers(0, 40))
         full_len = len(read) + ext_qs + ext_qe
         anchors = []
-        for y in range(0, len(read) - 256, 256):
+        for y in range(0, len(read) - rpl, rpl):
             x = int(y * (on_stop - on_start) / max(len(read), 1)) + int(rng.integers(-20, 21))
             rev = int(rng.integers(0, 2))
-            on_read = (full_len - (y + ext_qs) - 256) if rev else (y + ext_qs)
+            on_read = (full_len - (y + ext_qs) - rpl) if rev else (y + ext_qs)
             anchors.append((on_read, on_start + max(x, 0), rev))
         kind = k % 6
         t = IntervalTask(on_ref_start=on_start, on_ref_stop=on_stop, read_seq=read.tobytes(),
                          corridor=corridor.estimate_corridor(len(read), on_stop - on_start),
                          ext_qstart=ext_qs, ext_qend=ext_qe, full_read_length=full_len,
                          anchors=anchors if kind != 1 else [], realign=kind == 2,
-                         full_alignment=kind == 3 and L < 900, short_read=kind == 4)
+                         full_alignment=kind == 3 and L < 900, short_read=kind == 4, read_part_length=rpl)
         if kind == 5:
             t.corridor = 40       # far too narrow: forces retries with wider corridors
             t.anchors = []
