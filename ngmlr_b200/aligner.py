@@ -571,8 +571,12 @@ class B200Aligner:
         self.lib.ngmlr_b200_debug_set_arena_words(self.h, int(words))
 
     def debug_rampfree_problems(self):
-        """Test hook: problems filled by the ramp-free fill kernel since the context was created."""
+        """Test hook: problems filled by the ramp-free fill kernels since the context was created."""
         return int(self.lib.ngmlr_b200_debug_rampfree_problems(self.h))
+
+    def debug_rampfree2_problems(self):
+        """Test hook: of those, problems filled by the kernel with two rows per lane."""
+        return int(self.lib.ngmlr_b200_debug_rampfree2_problems(self.h))
 
     def set_small_batch_teams(self, on):
         """16-warp teams for batches of at most one problem per SM (default on); see ngmlr_b200_set_small_batch_teams."""

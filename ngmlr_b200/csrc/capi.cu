@@ -131,6 +131,15 @@ int ngmlr_b200_create(int gpu_id, const ngmlr_b200_scoring* s, ngmlr_b200_ctx** 
       return -1;
     }
   }
+  if (const char* e = getenv("NGMLR_B200_FILL_ROWS_PER_LANE")) {
+    if (!strcmp(e, "1")) ctx->rows_per_lane = 1;
+    else if (!strcmp(e, "2")) ctx->rows_per_lane = 2;
+    else {
+      g_create_error = std::string("ngmlr_b200: NGMLR_B200_FILL_ROWS_PER_LANE=") + e + ": expected 1 or 2";
+      ngmlr_b200_destroy(ctx);
+      return -1;
+    }
+  }
   if (const char* e = getenv("NGMLR_B200_RF_TEAM_CELLS")) ctx->rf_team_cells = strtoull(e, nullptr, 10);
   if (const char* e = getenv("NGMLR_B200_FILL_CTAS_PER_SM")) ctx->fill_ctas_cap = std::max(0, atoi(e));
   if (const char* e = getenv("NGMLR_B200_NO_CORRIDOR_PACKING")) ctx->no_corridor_packing = atoi(e);
@@ -237,8 +246,10 @@ int ngmlr_b200_debug_set_big_team(ngmlr_b200_ctx* ctx, long long cells, int widt
   return 0;
 }
 
-// Test hook: problems filled by the ramp-free kernel since the context was created.
+// Test hooks: problems filled by the ramp-free kernels since the context was created; of those, by the kernel with
+// two rows per lane.
 long long ngmlr_b200_debug_rampfree_problems(ngmlr_b200_ctx* ctx) { return ctx ? (long long)ctx->rf_problems : -1; }
+long long ngmlr_b200_debug_rampfree2_problems(ngmlr_b200_ctx* ctx) { return ctx ? (long long)ctx->rf2_problems : -1; }
 
 // force_team: -1 auto, 0 one warp per problem, 1 four-warp teams. Test / tuning hook.
 int ngmlr_b200_set_force_team(ngmlr_b200_ctx* ctx, int v) {
@@ -305,7 +316,9 @@ int ngmlr_b200_convex_debug_directions(ngmlr_b200_ctx* ctx, int i, uint8_t* dirs
   size_t row_base = 0;
   for (size_t b = 0; b < nblk; ++b) {
     const BlockRec& br = blocks[b];
-    const size_t nw = (size_t)((br.nsteps + 15) / 16) * 32;
+    const int sh = f.dir_shift;
+    const size_t stride = (size_t)32 << sh, ng = (size_t)((br.nsteps + 15) / 16);
+    const size_t nw = ng ? (ng - 1) * stride + 32 : 0;
     words.resize(nw);
     if (nw) CU(cudaMemcpy(words.data(), ctx->d_dir.p + br.word_off, nw * 4, cudaMemcpyDeviceToHost));
     for (int t = 0; t < 32; ++t) {
@@ -314,8 +327,8 @@ int ngmlr_b200_convex_debug_directions(ngmlr_b200_ctx* ctx, int i, uint8_t* dirs
       const int lo = std::max(offs[y], 0);
       const int hi = (int)std::min<long long>((long long)offs[y] + lens[y], d.ref_len);
       for (int x = lo; x < hi; ++x) {
-        const int s = x - br.base + t;
-        const uint32_t code = (words[(size_t)(s >> 4) * 32 + t] >> ((s & 15) * 2)) & 3u;
+        const int s = x - br.base + (t >> sh);
+        const uint32_t code = (words[(size_t)(s >> 4) * stride + t] >> ((s & 15) * 2)) & 3u;
         uint8_t v = OP_STOP;
         if (code == DIR_DIAG) v = qry[y] == ref[x] ? OP_EQ : OP_X;
         else if (code == DIR_I) v = OP_I;

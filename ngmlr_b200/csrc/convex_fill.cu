@@ -133,6 +133,91 @@ struct LaneState {
   int rel;      // x - xlo of the current step; inside the corridor iff (unsigned)rel < rlen
 };
 
+// One cell (x, y) at step s. `st` is the row's state (LaneState or RowState: lL, lRunF / lIsD or lRun / lDir, kS /
+// kStep, rel); dS = S of (x-1, y-1), {nU, nP} = U and run of (x, y-1), r = the column's reference byte, q = the row's
+// read byte. Returns the direction code; {S, U, P} is what the cell below sees as its up neighbour.
+template <bool RAW, bool ALL_ACTIVE, class Row>
+__device__ __forceinline__ uint32_t cell_update(Row& st, const Scoring& sc, const float dS, const float nU,
+                                                const uint32_t nP, const uint32_t r, const uint32_t q, const bool act,
+                                                const int t0rel, const int s, float& S, float& U, uint32_t& P) {
+  float dg = __fadd_rn(dS, sc.mis);
+  if (r == q) dg = __fadd_rn(dS, sc.mat);
+  // Outside the corridor the cell must degenerate to {0, 0, STOP}: a NaN maximum makes every
+  // equality below false, and fmaxf(NaN, 0) = 0 gives the score.
+  const float m0 = fmaxf(fmaxf(fmaxf(st.lL, 0.0f), dg), nU);
+  const float m = (ALL_ACTIVE || act) ? m0 : __int_as_float(0x7fffffff);
+  const bool eL = (m == st.lL), eU = (m == nU), eG = (m == dg);
+  S = ALL_ACTIVE ? m : fmaxf(m, 0.0f);  // STOP implies m == 0
+  uint32_t code;
+  float L;
+  if (RAW) {
+    const int upRaw = (int)(short)(nP & 0xffffu);
+    const uint32_t upDir = (nP >> 16) & 3u;
+    const bool rawHere = st.rel < t0rel;
+    const int upRun = (rawHere || upDir == DIR_I) ? upRaw : 0;
+    const int leftRun = (rawHere || st.lDir == DIR_D) ? st.lRun : 0;
+    // priority (:1232-1267): continue D, continue I, diagonal, open D, open I, STOP
+    const bool dc = eL && (leftRun > 0);
+    const bool ic = !dc && eU && (upRun > 0);
+    const bool gg = !dc && !ic && eG;
+    const bool resolved = dc || ic || gg;
+    const bool isD = dc || (!resolved && eL);
+    const bool isI = ic || (!resolved && !eL && eU);
+    int run = dc ? leftRun : (ic ? upRun : 0);
+    run = (isD || isI) ? run + 1 : 0;
+    run = (int)(short)run;  // MatrixElement::indelRun is a short
+    code = gg ? DIR_DIAG : (isI ? DIR_I : (isD ? DIR_D : DIR_STOP));
+    // what the neighbours will see: S + min(ext_min, gap_ext + run*decay), 0 if S == 0 (:666-676)
+    const float pen = fminf(sc.ext_min, __fadd_rn(sc.gap_ext, __fmul_rn((float)run, sc.decay)));
+    float e = __fadd_rn(S, pen);
+    if (S == 0.0f) e = 0.0f;
+    U = isI ? e : __fadd_rn(S, sc.open_read);
+    L = isD ? e : __fadd_rn(S, sc.open_ref);
+    P = (code << 16) | ((uint32_t)run & 0xffffu);
+    st.lRun = run;
+    st.lDir = code;
+  } else {
+    // Same priority chain as a 3-input predicate network (verified exhaustively):
+    //   D  <=>  eL && (lr || !((eU && ur) || eG))
+    //   I  <=>  !D && eU && (ur || !eG)
+    // with run lengths kept as floats (exact below 2^24; rows are < 32768 wide here).
+    const float upRunF = __uint_as_float(nP);
+    const bool lr = st.lIsD, ur = upRunF > 0.0f;  // the left cell's run is > 0 iff it is a deletion
+    const bool X = (eU & ur) | eG;  // bitwise on purpose: straight PLOP3s, no short-circuit
+    const bool pD = eL & (lr | !X);
+    const bool pI = (!pD) & eU & (ur | !eG);
+    code = eG ? DIR_DIAG : DIR_STOP;
+    if (pI) asm volatile("mad.lo.u32 %0, %1, 0, 1;" : "=r"(code) : "r"(code));
+    if (pD) asm volatile("mad.lo.u32 %0, %1, 0, 2;" : "=r"(code) : "r"(code));
+    // at most one of the two run counters is alive after this cell
+    // "zero, then an addition under the predicate" instead of add + select: the selects, compares and
+    // min/max of this loop all go through the half-rate ALU pipe, which is what binds the kernel; a
+    // predicated FADD runs on the FMA pipe (same for dg above and U / L below)
+    float newD = 0.0f, newI = 0.0f;
+    if (pD) asm volatile("add.rn.f32 %0, %1, 0f3F800000;" : "=f"(newD) : "f"(st.lRunF));
+    if (pI) asm volatile("add.rn.f32 %0, %1, 0f3F800000;" : "=f"(newI) : "f"(upRunF));
+    const float runF = __fadd_rn(newD, newI);
+    const float pen = fminf(sc.ext_min, __fadd_rn(sc.gap_ext, __fmul_rn(runF, sc.decay)));
+    // e = (S == 0) ? 0 : S + pen  as one exact fused op: S + pen * [S != 0]
+    float nz;
+    asm("set.ne.f32.f32 %0, %1, 0f00000000;" : "=f"(nz) : "f"(S));
+    U = __fadd_rn(S, sc.open_read);
+    L = __fadd_rn(S, sc.open_ref);
+    if (pI) asm volatile("fma.rn.f32 %0, %1, %2, %3;" : "=f"(U) : "f"(pen), "f"(nz), "f"(S));
+    if (pD) asm volatile("fma.rn.f32 %0, %1, %2, %3;" : "=f"(L) : "f"(pen), "f"(nz), "f"(S));
+    P = __float_as_uint(newI);
+    st.lRunF = newD;
+    st.lIsD = pD;
+  }
+  st.lL = L;
+  if (S > st.kS) {  // strict: first maximum in row-major order (:1165-1170)
+    // S + 0 == S bit for bit (S >= +0); as predicated FMA-pipe instructions instead of two selects
+    asm volatile("add.rn.f32 %0, %1, 0f00000000;" : "=f"(st.kS) : "f"(S));
+    asm volatile("mad.lo.s32 %0, %1, 1, 0;" : "=r"(st.kStep) : "r"(s));
+  }
+  return code;
+}
+
 // 16 steps of one lane: cells (x, y) with x = the lane's column at step 16 g + k. `iop` and `dwp` address the
 // chunk's staging records and the lane's direction word of group 0. ALL_ACTIVE: every lane of the warp stays
 // inside its corridor row for all 16 steps (no masking at all: the common case away from a block's wavefront ends).
@@ -168,86 +253,14 @@ __device__ __forceinline__ void fill_group(LaneState& st, const Scoring& sc, uin
       const bool act = ALL_ACTIVE ? true : ((unsigned)st.rel < rlen);
       uint32_t r = v.w;
       if (SELF_REF && !act) r = __ldg(ref + min((unsigned)(s - colbase), ref_len));
-      float dg = __fadd_rn(st.dS, sc.mis);
-      if (r == q) dg = __fadd_rn(st.dS, sc.mat);
+      float S, U;
+      uint32_t P;
+      const uint32_t code = cell_update<RAW, ALL_ACTIVE>(st, sc, st.dS, nU, v.z, r, q, act, t0rel, s, S, U, P);
       st.dS = nS;
-      // Outside the corridor the cell must degenerate to {0, 0, STOP}: a NaN maximum makes every
-      // equality below false, and fmaxf(NaN, 0) = 0 gives the score.
-      const float m0 = fmaxf(fmaxf(fmaxf(st.lL, 0.0f), dg), nU);
-      const float m = (ALL_ACTIVE || act) ? m0 : __int_as_float(0x7fffffff);
-      const bool eL = (m == st.lL), eU = (m == nU), eG = (m == dg);
-      const float S = ALL_ACTIVE ? m : fmaxf(m, 0.0f);  // STOP implies m == 0
-      uint32_t code;
-      float U, L;
-      if (RAW) {
-        const uint32_t nP = v.z;
-        const int upRaw = (int)(short)(nP & 0xffffu);
-        const uint32_t upDir = (nP >> 16) & 3u;
-        const bool rawHere = st.rel < t0rel;
-        const int upRun = (rawHere || upDir == DIR_I) ? upRaw : 0;
-        const int leftRun = (rawHere || st.lDir == DIR_D) ? st.lRun : 0;
-        // priority (:1232-1267): continue D, continue I, diagonal, open D, open I, STOP
-        const bool dc = eL && (leftRun > 0);
-        const bool ic = !dc && eU && (upRun > 0);
-        const bool gg = !dc && !ic && eG;
-        const bool resolved = dc || ic || gg;
-        const bool isD = dc || (!resolved && eL);
-        const bool isI = ic || (!resolved && !eL && eU);
-        int run = dc ? leftRun : (ic ? upRun : 0);
-        run = (isD || isI) ? run + 1 : 0;
-        run = (int)(short)run;  // MatrixElement::indelRun is a short
-        code = gg ? DIR_DIAG : (isI ? DIR_I : (isD ? DIR_D : DIR_STOP));
-        // what the neighbours will see: S + min(ext_min, gap_ext + run*decay), 0 if S == 0 (:666-676)
-        const float pen = fminf(sc.ext_min, __fadd_rn(sc.gap_ext, __fmul_rn((float)run, sc.decay)));
-        float e = __fadd_rn(S, pen);
-        if (S == 0.0f) e = 0.0f;
-        U = isI ? e : __fadd_rn(S, sc.open_read);
-        L = isD ? e : __fadd_rn(S, sc.open_ref);
-        st.oP = (code << 16) | ((uint32_t)run & 0xffffu);
-        st.lRun = run;
-        st.lDir = code;
-      } else {
-        // Same priority chain as a 3-input predicate network (verified exhaustively):
-        //   D  <=>  eL && (lr || !((eU && ur) || eG))
-        //   I  <=>  !D && eU && (ur || !eG)
-        // with run lengths kept as floats (exact below 2^24; rows are < 32768 wide here).
-        const float upRunF = __uint_as_float(v.z);
-        const bool lr = st.lIsD, ur = upRunF > 0.0f;  // the left cell's run is > 0 iff it is a deletion
-        const bool X = (eU & ur) | eG;  // bitwise on purpose: straight PLOP3s, no short-circuit
-        const bool pD = eL & (lr | !X);
-        const bool pI = (!pD) & eU & (ur | !eG);
-        code = eG ? DIR_DIAG : DIR_STOP;
-        if (pI) asm volatile("mad.lo.u32 %0, %1, 0, 1;" : "=r"(code) : "r"(code));
-        if (pD) asm volatile("mad.lo.u32 %0, %1, 0, 2;" : "=r"(code) : "r"(code));
-        // at most one of the two run counters is alive after this cell
-        // "zero, then an addition under the predicate" instead of add + select: the selects, compares and
-        // min/max of this loop all go through the half-rate ALU pipe, which is what binds the kernel; a
-        // predicated FADD runs on the FMA pipe (same for dg above and U / L below)
-        float newD = 0.0f, newI = 0.0f;
-        if (pD) asm volatile("add.rn.f32 %0, %1, 0f3F800000;" : "=f"(newD) : "f"(st.lRunF));
-        if (pI) asm volatile("add.rn.f32 %0, %1, 0f3F800000;" : "=f"(newI) : "f"(upRunF));
-        const float runF = __fadd_rn(newD, newI);
-        const float pen = fminf(sc.ext_min, __fadd_rn(sc.gap_ext, __fmul_rn(runF, sc.decay)));
-        // e = (S == 0) ? 0 : S + pen  as one exact fused op: S + pen * [S != 0]
-        float nz;
-        asm("set.ne.f32.f32 %0, %1, 0f00000000;" : "=f"(nz) : "f"(S));
-        U = __fadd_rn(S, sc.open_read);
-        L = __fadd_rn(S, sc.open_ref);
-        if (pI) asm volatile("fma.rn.f32 %0, %1, %2, %3;" : "=f"(U) : "f"(pen), "f"(nz), "f"(S));
-        if (pD) asm volatile("fma.rn.f32 %0, %1, %2, %3;" : "=f"(L) : "f"(pen), "f"(nz), "f"(S));
-        st.oP = __float_as_uint(newI);
-        st.lRunF = newD;
-        st.lIsD = pD;
-      }
       st.oS = S;
       st.oU = U;
+      st.oP = P;
       st.oC = r;
-      st.lL = L;
-      if (S > st.kS) {  // strict: first maximum in row-major order (:1165-1170)
-        // S + 0 == S bit for bit (S >= +0); as predicated FMA-pipe instructions instead of two selects
-        asm volatile("add.rn.f32 %0, %1, 0f00000000;" : "=f"(st.kS) : "f"(S));
-        asm volatile("mad.lo.s32 %0, %1, 1, 0;" : "=r"(st.kStep) : "r"(s));
-      }
       dw = __funnelshift_r(dw, code, 2);
 #if FILL_LANE0_LDS
       if (is31) iop[1] = make_uint4(__float_as_uint(st.oS), __float_as_uint(st.oU), st.oP, st.oC);
@@ -588,6 +601,7 @@ convex_fill_kernel(const FillParams p) {
       o.best_y = bestY;
       o.status = status;
       o.cells = cells;
+      o.dir_shift = 0;
       p.out[ai] = o;
     }
   }
@@ -655,18 +669,23 @@ __device__ __forceinline__ void rf_cols(int xlo, int xhi, unsigned rlen, int lan
   E = max(e, e1);
 }
 
-// Origin and entry steps of block b. L: end of the lane's previous range (RF_NONE: none); R: earliest entry;
-// O_min: the hand-off bound.
+// Origin and entry step of a block from the lane's columns [A, ...). L: end of the lane's previous range (RF_NONE:
+// none); R: earliest entry; O_min: the hand-off bound.
+__device__ __forceinline__ void rf_origin(int lane, int A, int L, int R, int O_min, int& O, int& sw) {
+  const int from = max(L, R);
+  const int need = A == INT_MAX ? INT_MIN : ((from + 15) & ~15) - lane - A;
+  O = max(O_min, __reduce_max_sync(FULL, need));
+  sw = A == INT_MAX ? RF_NONE : ((O + lane + A) & ~15);
+}
+
+// Origin and entry steps of block b (see rf_origin).
 __device__ __forceinline__ void rf_place(const CorridorView& cv, int b, int lane, int H, int ref_len, int L, int R,
                                          int O_min, int& xlo, unsigned& rlen, int& A, int& E, int& O, int& sw) {
   int off, len, xhi;
   load_corridor_rows(cv, b, lane, H, off, len);
   row_span(off, len, ref_len, xlo, xhi, rlen);
   rf_cols(xlo, xhi, rlen, lane, A, E);
-  const int from = max(L, R);
-  const int need = A == INT_MAX ? INT_MIN : ((from + 15) & ~15) - lane - A;
-  O = max(O_min, __reduce_max_sync(FULL, need));
-  sw = A == INT_MAX ? RF_NONE : ((O + lane + A) & ~15);
+  rf_origin(lane, A, L, R, O_min, O, sw);
 }
 
 constexpr int RF_CHUNK = 64;                  // steps staged through shared memory at a time
@@ -674,6 +693,20 @@ constexpr int RF_RING = 32 + 2 * RF_CHUNK;    // hand-off spacing of consecutive
 
 // the earliest entry into the block after one whose last lane enters at step swmax
 __device__ __forceinline__ int rf_next_entry(int swmax) { return ((swmax + RF_CHUNK) / RF_CHUNK + 1) * RF_CHUNK; }
+
+// A strip slot of the SM the calling CTA runs on (short-lived CTAs, see convex_fill_kernel): SM * FILL_SM_SLOTS + slot.
+__device__ __forceinline__ int take_sm_slot(const FillParams& p) {
+  unsigned smid;
+  asm("mov.u32 %0, %%smid;" : "=r"(smid));
+  int got = -1;
+  for (;;) {
+    for (int b = 0; b < p.sm_slot_count && got < 0; ++b)
+      if (!(atomicOr(p.sm_slots + smid, 1u << b) & (1u << b))) got = b;
+    if (got >= 0) break;
+    __nanosleep(2000);
+  }
+  return (int)smid * FILL_SM_SLOTS + got;
+}
 
 template <bool RAW, bool PERSIST>
 __global__ void __launch_bounds__(FILL_WARPS_PER_CTA * 32, FILL_CTAS_PER_SM)
@@ -691,18 +724,7 @@ convex_fill_rf_kernel(const FillParams p) {
   const int lane = threadIdx.x & 31;
   const int wib = threadIdx.x >> 5;
   if (!PERSIST) {  // as in convex_fill_kernel; the slot is given back from s_slot (no registers held meanwhile)
-    if (threadIdx.x == 0) {
-      unsigned smid;
-      asm("mov.u32 %0, %%smid;" : "=r"(smid));
-      int got = -1;
-      for (;;) {
-        for (int b = 0; b < p.sm_slot_count && got < 0; ++b)
-          if (!(atomicOr(p.sm_slots + smid, 1u << b) & (1u << b))) got = b;
-        if (got >= 0) break;
-        __nanosleep(2000);
-      }
-      s_slot = (int)smid * FILL_SM_SLOTS + got;
-    }
+    if (threadIdx.x == 0) s_slot = take_sm_slot(p);
     __syncthreads();
   }
   const int cta_slot = PERSIST ? (int)blockIdx.x : s_slot;
@@ -1013,6 +1035,509 @@ convex_fill_rf_kernel(const FillParams p) {
       o.best_y = bestY;
       o.status = status;
       o.cells = cells;
+      o.dir_shift = 0;
+      p.out[ai] = o;
+    }
+    __syncwarp();
+  }
+  if (!PERSIST) {
+    __syncthreads();
+    if (threadIdx.x == 0) atomicAnd(p.sm_slots + s_slot / FILL_SM_SLOTS, ~(1u << (s_slot % FILL_SM_SLOTS)));
+  }
+}
+
+// ---- ramp-free schedule, two rows per lane -------------------------------------------------------------------------
+// The schedule above with 64-row blocks: lane t owns rows 64b + 2t (its first row) and 64b + 2t + 1 (its second) and
+// evaluates column x of both at warp step O_b + t + x, the first row before the second. The first row takes its up and
+// diagonal neighbours from lane t-1's second row through the shuffle, as before; the second row takes them from the
+// first row's fresh cell and from its cell of the step before, in registers, and both rows use the same reference
+// byte. Every shuffle, strip hand-off, loop step and reference byte therefore serves two cells, and the per-block work
+// (placement, masked groups at the block switch) is spread over 64 rows.
+// Lane t's columns [A, E) of a block cover its two rows and the row below (lane t+1's first row), one
+// out-of-corridor step first; lane 31's reach the block's rightmost column. The placement rules are those above.
+// Where the first row is outside its corridor lane t-1 may have left the block, so the lane loads the reference byte
+// itself there (its second row may still be inside).
+// Direction words: group g of the warp's steps is a line of 64 words, lane t's two rows at 64 g + 2t and 64 g + 2t + 1
+// (one 8-byte store per lane). The two 32-row halves of a block keep a BlockRec each: half h at word_off + 32 h with
+// base - 16 h, so that cell (x, 32 (2b + h) + j) lies at step x - base + (j >> 1) (FillOut::dir_shift = 1).
+
+// What one row of a lane carries from step to step (the fields of LaneState that belong to a row).
+struct RowState {
+  float lL;
+  float lRunF;
+  bool lIsD;
+  int lRun;
+  uint32_t lDir;
+  float kS;
+  int kStep;
+  int rel;
+};
+
+struct Lane2State {
+  float oS, oU;  // the second row's cell: what lane t+1 (or lane 0 of the next block) reads, as in LaneState
+  uint32_t oP, oC;
+  float dS;      // S of (x-1, first row - 1)
+  float dS2;     // S of (x-1, first row)
+  RowState a, b; // first and second row
+};
+
+struct RowGeom {
+  unsigned rlen;
+  uint32_t q;
+  int t0rel;
+};
+
+__device__ __forceinline__ void row_init(RowState& r, const Scoring& sc) {
+  r.lL = sc.open_ref;
+  r.lRunF = 0.0f;
+  r.lIsD = false;
+  r.lRun = 0;
+  r.lDir = DIR_STOP;
+  r.kS = 0.0f;
+  r.kStep = -1;
+  r.rel = 0;
+}
+
+// fill_group for two rows per lane; `dwp` addresses the lane's pair of direction words of group 0.
+template <bool RAW, bool ALL_ACTIVE, int GPC, bool SELF_REF = false>
+__device__ __forceinline__ void fill_group2(Lane2State& st, const Scoring& sc, uint4* const io_s, uint2* const dwp,
+                                            const int g, const RowGeom& ga, const RowGeom& gb, const bool is31,
+                                            const int src_lane, const uint8_t* ref = nullptr, int colbase = 0,
+                                            unsigned ref_len = 0) {
+  uint4* iop = io_s + ((g % GPC) << 5);
+  uint32_t dwa = 0, dwb = 0;
+  {
+#pragma unroll 2
+    for (int k = 0; k < 16; ++k) {
+      const int s = (g << 4) + k;
+      uint4 v;
+      v.x = __float_as_uint(__shfl_sync(FULL, st.oS, src_lane));
+      v.y = __float_as_uint(__shfl_sync(FULL, st.oU, src_lane));
+      v.z = __shfl_sync(FULL, st.oP, src_lane);
+      v.w = __shfl_sync(FULL, st.oC, src_lane);
+      const float nS = __uint_as_float(v.x), nU = __uint_as_float(v.y);
+      const bool actA = ALL_ACTIVE ? true : ((unsigned)st.a.rel < ga.rlen);
+      const bool actB = ALL_ACTIVE ? true : ((unsigned)st.b.rel < gb.rlen);
+      uint32_t r = v.w;
+      if (SELF_REF && !actA) r = __ldg(ref + min((unsigned)(s - colbase), ref_len));
+      float SA, UA, SB, UB;
+      uint32_t PA, PB;
+      const uint32_t ca = cell_update<RAW, ALL_ACTIVE>(st.a, sc, st.dS, nU, v.z, r, ga.q, actA, ga.t0rel, s, SA, UA, PA);
+      st.dS = nS;
+      const uint32_t cb = cell_update<RAW, ALL_ACTIVE>(st.b, sc, st.dS2, UA, PA, r, gb.q, actB, gb.t0rel, s, SB, UB, PB);
+      st.dS2 = SA;
+      st.oS = SB;
+      st.oU = UB;
+      st.oP = PB;
+      st.oC = r;
+      dwa = __funnelshift_r(dwa, ca, 2);
+      dwb = __funnelshift_r(dwb, cb, 2);
+      if (is31) {
+        iop[1] = make_uint4(__float_as_uint(st.oS), __float_as_uint(st.oU), st.oP, st.oC);
+        const uint4 t = iop[2];
+        st.oS = __uint_as_float(t.x);
+        st.oU = __uint_as_float(t.y);
+        st.oP = t.z;
+        st.oC = t.w;
+      }
+      iop += 2;
+      if (!ALL_ACTIVE || RAW) {
+        ++st.a.rel;
+        ++st.b.rel;
+      }
+    }
+  }
+  if (ALL_ACTIVE && !RAW) {
+    st.a.rel += 16;
+    st.b.rel += 16;
+  }
+  if (ALL_ACTIVE || (st.a.rel > 0 && st.a.rel - 16 < (int)ga.rlen) || (st.b.rel > 0 && st.b.rel - 16 < (int)gb.rlen))
+    dwp[(size_t)g * 32] = make_uint2(dwa, dwb);
+}
+
+// Corridor rows 64b + 2 lane and 64b + 2 lane + 1 of the whole warp; rows >= H read as {0, 0}.
+__device__ __forceinline__ void load_row_pair(const CorridorView& cv, int b, int lane, int H, int& offA, int& lenA,
+                                              int& offB, int& lenB) {
+  int o0, l0, o1, l1;
+  load_corridor_rows(cv, 2 * b, lane, H, o0, l0);
+  load_corridor_rows(cv, 2 * b + 1, lane, H, o1, l1);
+  const int sa = (2 * lane) & 31, sb = sa + 1;
+  const bool hi = lane >= 16;
+  const int oa0 = __shfl_sync(FULL, o0, sa), oa1 = __shfl_sync(FULL, o1, sa);
+  const int la0 = __shfl_sync(FULL, l0, sa), la1 = __shfl_sync(FULL, l1, sa);
+  const int ob0 = __shfl_sync(FULL, o0, sb), ob1 = __shfl_sync(FULL, o1, sb);
+  const int lb0 = __shfl_sync(FULL, l0, sb), lb1 = __shfl_sync(FULL, l1, sb);
+  offA = hi ? oa1 : oa0;
+  lenA = hi ? la1 : la0;
+  offB = hi ? ob1 : ob0;
+  lenB = hi ? lb1 : lb0;
+}
+
+// Lane t's columns [A, E) of a 64-row block (A = INT_MAX: none), from its two rows and the row below.
+__device__ __forceinline__ void rf2_cols(int xloA, int xhiA, unsigned rlenA, int xloB, int xhiB, unsigned rlenB,
+                                         int lane, int& A, int& E) {
+  const int aA = rlenA ? xloA : INT_MAX, eA = rlenA ? xhiA : INT_MIN;
+  const int aB = rlenB ? xloB : INT_MAX, eB = rlenB ? xhiB : INT_MIN;
+  const int e = max(eA, eB);
+  int a1 = __shfl_down_sync(FULL, aA, 1), e1 = __shfl_down_sync(FULL, eA, 1);
+  const int emax = __reduce_max_sync(FULL, e);
+  if (lane == 31) {
+    a1 = INT_MAX;
+    e1 = emax;
+  }
+  const int amin = min(min(aA, aB), a1);
+  A = amin == INT_MAX ? INT_MAX : amin - 1;
+  E = max(e, e1);
+}
+
+// rf_place for 64-row block b.
+__device__ __forceinline__ void rf2_place(const CorridorView& cv, int b, int lane, int H, int ref_len, int L, int R,
+                                          int O_min, int& xloA, unsigned& rlenA, int& xloB, unsigned& rlenB, int& A,
+                                          int& E, int& O, int& sw) {
+  int offA, lenA, offB, lenB, xhiA, xhiB;
+  load_row_pair(cv, b, lane, H, offA, lenA, offB, lenB);
+  row_span(offA, lenA, ref_len, xloA, xhiA, rlenA);
+  row_span(offB, lenB, ref_len, xloB, xhiB, rlenB);
+  rf2_cols(xloA, xhiA, rlenA, xloB, xhiB, rlenB, lane, A, E);
+  rf_origin(lane, A, L, R, O_min, O, sw);
+}
+
+template <bool RAW, bool PERSIST>
+__global__ void __launch_bounds__(FILL_WARPS_PER_CTA * 32, FILL_RF2_CTAS_PER_SM)
+convex_fill_rf2_kernel(const FillParams p) {
+  constexpr int WARPS = FILL_WARPS_PER_CTA;
+  constexpr int CHUNK = RF_CHUNK;
+  constexpr int GPC = CHUNK / 16;
+  __shared__ uint4 s_io[WARPS][2 * (CHUNK + 1)];
+  __shared__ int s_slot;
+  __shared__ RfFrame s_f0[WARPS], s_f31[WARPS], s_nx[WARPS];  // as in convex_fill_rf_kernel, blk counts 64-row blocks
+  __shared__ int4 s_nrow[WARPS][2][32];  // the lane's two rows of the next block: {rel at entry, rlen, q}
+  __shared__ int4 s_cur[WARPS][32];      // {O, y of the first row} of the lane's current rows, L, its cells
+  __shared__ float4 s_bestl[WARPS][32];  // the lane's best cell of its finished rows {S, x, y}
+  __shared__ RfWarp s_w[WARPS];          // word_off: group g of the warp's steps at word_off + 64 g
+  const int lane = threadIdx.x & 31;
+  const int wib = threadIdx.x >> 5;
+  if (!PERSIST) {
+    if (threadIdx.x == 0) s_slot = take_sm_slot(p);
+    __syncthreads();
+  }
+  const int cta_slot = PERSIST ? (int)blockIdx.x : s_slot;
+  uint4* const io_s = s_io[wib];
+  uint4* const strip = reinterpret_cast<uint4*>(p.bnd) + (size_t)(cta_slot * WARPS + wib) * p.bnd_stride + STRIP_PAD;
+  const Scoring sc = p.sc;
+  const uint32_t empty_pack = RAW ? (DIR_STOP << 16) : 0u;
+  const uint4 EMPTY = make_uint4(0u, __float_as_uint(sc.open_read), empty_pack, 0u);
+  const bool is0 = lane == 0, is31 = lane == 31;
+  const int src_lane = (lane + 31) & 31;
+  RfWarp& ws = s_w[wib];
+
+  for (int taken = 0; PERSIST || taken < p.problems_per_cta; ++taken) {
+    int w = 0;
+    if (is0) w = atomicAdd(p.work_counter, 1);
+    w = __shfl_sync(FULL, w, 0) + p.first;
+    if (w >= p.last) break;
+    const int ai = p.order[w];
+    auto corridor = [&]() {
+      CorridorView cv;
+      cv.bind(p.c_off, p.c_len, p.c_blkbase, p.c_delta, p.desc[ai]);
+      return cv;
+    };
+    const uint8_t* __restrict__ ref = p.seq + p.desc[ai].ref_off;
+    const unsigned ref_len = (unsigned)p.desc[ai].ref_len;
+    int status = ST_OK;
+
+    // Pass 1: the warp's schedule (the same placements as pass 2 makes) -> its number of steps.
+    {
+      const CorridorView cv = corridor();
+      const int H = p.desc[ai].height, nblk = (H + 63) >> 6;
+      int L = RF_NONE, R = 0, O_last = RF_NONE;
+      for (int b = 0; b < nblk; ++b) {
+        int xloA, xloB, A, E, O, sw;
+        unsigned rlA, rlB;
+        rf2_place(cv, b, lane, H, (int)ref_len, L, R, O_last == RF_NONE ? INT_MIN : O_last + RF_RING, xloA, rlA, xloB,
+                  rlB, A, E, O, sw);
+        if (__any_sync(FULL, sw != RF_NONE)) O_last = O;
+        if (sw != RF_NONE) L = O + lane + E;
+        R = rf_next_entry(__reduce_max_sync(FULL, sw != RF_NONE ? sw : R - 1));
+      }
+      const int T = max(0, __reduce_max_sync(FULL, L));
+      const int G = (T + 15) >> 4;
+      unsigned long long wo = 0;
+      if (is0) wo = atomicAdd(p.dir_alloc, (unsigned long long)G * 64ull);
+      wo = __shfl_sync(FULL, wo, 0);
+      if (wo + (unsigned long long)G * 64ull > p.dir_capacity) status = ST_DIR_OVERFLOW;
+      if (is0) {
+        ws.word_off = wo;
+        ws.G = G;
+        ws.next_b = 0;
+        ws.R = 0;
+        ws.O_last = RF_NONE;
+        ws.firstX = 0;
+        ws.firstY = -1;
+        RfFrame none;
+        none.blk = -1;
+        none.O = none.wlo = none.whi = none.a31 = none.e31 = 0;
+        none.sw0 = none.sw31 = RF_NONE;
+        none.swmax = 0;
+        s_f0[wib] = none;
+        s_f31[wib] = none;
+        s_nx[wib] = none;
+      }
+      s_cur[wib][lane] = make_int4(0, 0, RF_NONE, 0);
+      s_bestl[wib][lane] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+      __syncwarp();
+    }
+    // every allocation of the arena is a multiple of 32 words: the pair is 8-byte aligned
+    uint2* __restrict__ dwp = reinterpret_cast<uint2*>(p.dir + ws.word_off) + lane;
+
+    // Pass 2.
+    Lane2State st;
+    st.oS = 0.0f;
+    st.oU = sc.open_read;
+    st.oP = empty_pack;
+    st.oC = 0u;
+    st.dS = 0.0f;
+    st.dS2 = 0.0f;
+    row_init(st.a, sc);
+    row_init(st.b, sc);
+    RowGeom ga, gb;  // before its first rows a lane is outside every corridor
+    ga.rlen = gb.rlen = 0;
+    ga.q = gb.q = 0x100u;
+    ga.t0rel = gb.t0rel = 0;
+    int sw = RF_NONE;
+
+    // the lane's best cell so far into s_bestl: the later row wins only with a larger score (row-major order); both
+    // trackers go on from it
+    auto take_best = [&](const int4& me) {
+      const bool second = st.b.kS > st.a.kS;
+      const int ks = second ? st.b.kStep : st.a.kStep;
+      const float kS = second ? st.b.kS : st.a.kS;
+      if (ks >= 0)
+        s_bestl[wib][lane] = make_float4(kS, __int_as_float(ks - me.x - lane), __int_as_float(me.y + (second ? 1 : 0)),
+                                         0.0f);
+      st.a.kS = st.b.kS = kS;
+      st.a.kStep = st.b.kStep = -1;
+    };
+
+    auto place = [&]() {
+      const CorridorView cv = corridor();
+      const AlnDesc* dp = p.desc + ai;
+      const int H = dp->height;
+      const int b = ws.next_b, R = ws.R, O_last = ws.O_last;
+      int4 me = s_cur[wib][lane];
+      int xloA, xloB, A, E, O, swl;
+      unsigned rlA, rlB;
+      rf2_place(cv, b, lane, H, (int)ref_len, me.z, R, O_last == RF_NONE ? INT_MIN : O_last + RF_RING, xloA, rlA, xloB,
+                rlB, A, E, O, swl);
+      const bool any = __any_sync(FULL, swl != RF_NONE);
+      if (swl != RF_NONE) me.z = O + lane + E;
+      me.w += (int)(rlA + rlB);
+      const int swmax = __reduce_max_sync(FULL, swl != RF_NONE ? swl : R - 1);
+      const int y = (b << 6) + 2 * lane;
+      const int4 na = make_int4(swl - (O + lane + xloA), (int)rlA, y < H ? (int)p.seq[dp->qry_off + y] : 0x100, 0);
+      const int4 nb2 = make_int4(swl - (O + lane + xloB), (int)rlB, y + 1 < H ? (int)p.seq[dp->qry_off + y + 1] : 0x100, 0);
+      // the first row of the block with a cell (rows 2t, 2t + 1 of lane t in row-major order)
+      const int key = rlA ? 2 * lane : (rlB ? 2 * lane + 1 : INT_MAX);
+      const int kmin = __reduce_min_sync(FULL, key);
+      const int fx = __shfl_sync(FULL, rlA ? xloA : xloB, (kmin >> 1) & 31);
+      // lane 31's columns of block b-1: what lane 0 of block b reads from the strip
+      int wlo = 0, whi = 0;
+      if (b > 0) {
+        int poA, plA, poB, plB, pxloA, pxhiA, pxloB, pxhiB, pA, pE;
+        unsigned prlA, prlB;
+        load_row_pair(cv, b - 1, lane, H, poA, plA, poB, plB);
+        row_span(poA, plA, (int)ref_len, pxloA, pxhiA, prlA);
+        row_span(poB, plB, (int)ref_len, pxloB, pxhiB, prlB);
+        rf2_cols(pxloA, pxhiA, prlA, pxloB, pxhiB, prlB, lane, pA, pE);
+        pA = __shfl_sync(FULL, pA, 31);
+        pE = __shfl_sync(FULL, pE, 31);
+        if (pA != INT_MAX) {
+          wlo = pA;
+          whi = pE;
+        }
+      }
+      const int g0 = __reduce_min_sync(FULL, swl != RF_NONE ? swl : INT_MAX);
+      const int end = __reduce_max_sync(FULL, swl != RF_NONE ? O + lane + E : INT_MIN);
+      const int a31 = __shfl_sync(FULL, A, 31), e31 = __shfl_sync(FULL, E, 31);
+      const int sw0 = __shfl_sync(FULL, swl, 0), sw31 = __shfl_sync(FULL, swl, 31);
+      s_cur[wib][lane] = me;
+      s_nrow[wib][0][lane] = na;
+      s_nrow[wib][1][lane] = nb2;
+      sw = swl;
+      __syncwarp();
+      if (is0) {
+        const int nblk32 = (H + 31) >> 5;
+        for (int h = 0; h < 2 && 2 * b + h < nblk32; ++h) {
+          BlockRec br;
+          br.word_off = ws.word_off + (any ? (unsigned long long)(g0 >> 4) * 64ull : 0ull) + 32ull * h;
+          br.base = any ? g0 - O - 16 * h : 0;
+          br.nsteps = any ? end - g0 : 0;
+          p.blocks[dp->blk_off + 2 * b + h] = br;
+        }
+        RfFrame f;
+        f.blk = b;
+        f.O = O;
+        f.wlo = wlo;
+        f.whi = whi;
+        f.a31 = a31;
+        f.e31 = e31;
+        f.sw0 = sw0;
+        f.sw31 = sw31;
+        f.swmax = swmax;
+        s_nx[wib] = f;
+        ws.next_b = b + 1;
+        ws.R = rf_next_entry(swmax);
+        if (any) ws.O_last = O;
+        if (kmin != INT_MAX && ws.firstY < 0) {
+          ws.firstY = (b << 6) + kmin;
+          ws.firstX = fx;
+        }
+      }
+      __syncwarp();
+    };
+    // as in convex_fill_rf_kernel
+    uint4 pa = EMPTY, pb = EMPTY;
+    auto stage = [&](int kk) {
+      const RfFrame* n = &s_nx[wib];
+      const RfFrame* f = &s_f0[wib];
+      const int nblk_ = n->blk, nsw0 = n->sw0, fblk = f->blk;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int sigma = kk * CHUNK + lane + 32 * h;
+        const bool in_n = nblk_ >= 0 && nsw0 != RF_NONE && sigma >= nsw0;
+        const RfFrame* fr = in_n ? n : f;
+        const int col = sigma - fr->O;
+        uint4 rec = EMPTY;
+        if (in_n || fblk >= 0) {
+          if (col >= fr->wlo && col < fr->whi) rec = ld_strip(strip + col);
+          rec.w = (unsigned)col < ref_len ? __ldg(ref + col) : 0u;
+        }
+        if (h == 0) pa = rec;
+        else pb = rec;
+      }
+    };
+
+    const int nchunks = status == ST_OK ? (ws.G + GPC - 1) / GPC : 0;
+    if (nchunks > 0) {
+      place();
+      stage(0);
+    }
+    for (int c = 0; c < nchunks; ++c) {
+      for (;;) {
+        const RfFrame n = s_nx[wib];
+        if (n.blk < 0 || n.swmax >= c * CHUNK) break;
+        __syncwarp();
+        if (is0) {
+          if (n.sw0 != RF_NONE) s_f0[wib] = n;
+          if (n.sw31 != RF_NONE) s_f31[wib] = n;
+          s_nx[wib].blk = -1;
+        }
+        __syncwarp();
+        if (ws.next_b < ((p.desc[ai].height + 63) >> 6)) place();
+        else sw = RF_NONE;
+      }
+      io_s[2 * lane] = pa;
+      io_s[2 * (lane + 32)] = pb;
+      __syncwarp();
+      if (is31) {
+        const uint4 t = io_s[0];
+        st.oS = __uint_as_float(t.x);
+        st.oU = __uint_as_float(t.y);
+        st.oP = t.z;
+        st.oC = t.w;
+      }
+      if (c + 1 < nchunks) stage(c + 1);
+      const int g_end = min(ws.G, (c + 1) * GPC);
+      for (int g = c * GPC; g < g_end; ++g) {
+        if ((g << 4) == sw) {  // this lane enters its rows of the next block
+          int4 me = s_cur[wib][lane];
+          take_best(me);
+          const int4 na = s_nrow[wib][0][lane], nb2 = s_nrow[wib][1][lane];
+          st.a.rel = na.x;
+          ga.rlen = (unsigned)na.y;
+          ga.q = (uint32_t)na.z;
+          ga.t0rel = na.y > 12 ? na.y - 12 : 0;
+          st.b.rel = nb2.x;
+          gb.rlen = (unsigned)nb2.y;
+          gb.q = (uint32_t)nb2.z;
+          gb.t0rel = nb2.y > 12 ? nb2.y - 12 : 0;
+          me.x = s_nx[wib].O;
+          me.y = (s_nx[wib].blk << 6) + 2 * lane;
+          s_cur[wib][lane] = me;
+          sw = RF_NONE;
+        }
+        const bool all_active = __all_sync(FULL, st.a.rel >= 0 && st.a.rel + 15 < (int)ga.rlen && st.b.rel >= 0 &&
+                                                     st.b.rel + 15 < (int)gb.rlen);
+        if (all_active) {
+          fill_group2<RAW, true, GPC>(st, sc, io_s, dwp, g, ga, gb, is31, src_lane);
+        } else {
+          fill_group2<RAW, false, GPC, true>(st, sc, io_s, dwp, g, ga, gb, is31, src_lane, ref,
+                                              s_cur[wib][lane].x + lane, ref_len);
+        }
+      }
+      __syncwarp();
+      // flush lane 31's records of this chunk that lie in its columns of the block it was in
+      {
+        const RfFrame* n = &s_nx[wib];
+        const RfFrame* f = &s_f31[wib];
+        const int done = (g_end - c * GPC) << 4;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int j = lane + 32 * h;
+          const int sigma = c * CHUNK + j;
+          const bool in_n = n->blk >= 0 && n->sw31 != RF_NONE && sigma >= n->sw31;
+          const RfFrame* fr = in_n ? n : f;
+          const int x = sigma - fr->O - 31;
+          if (j < done && (in_n || f->blk >= 0) && x >= fr->a31 && x < fr->e31) st_strip(strip + x, io_s[2 * j + 1]);
+        }
+      }
+      __syncwarp();
+    }
+    const int4 me = s_cur[wib][lane];
+    take_best(me);
+    const float4 bl = s_bestl[wib][lane];
+    float bestS = bl.x;
+    int bestX = __float_as_int(bl.y), bestY = __float_as_int(bl.z);
+    unsigned long long cells = (unsigned)me.w;
+    // blocks the schedule never reached have no cells
+    if (is0 && status == ST_OK)
+      for (int b = 2 * ws.next_b; b < ((p.desc[ai].height + 31) >> 5); ++b) {
+        BlockRec br;
+        br.word_off = ws.word_off;
+        br.base = 0;
+        br.nsteps = 0;
+        p.blocks[p.desc[ai].blk_off + b] = br;
+      }
+
+    // first maximum in row-major order across lanes: larger score, then smaller y, then smaller x
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      const float s2 = __shfl_xor_sync(FULL, bestS, o);
+      const int y2 = __shfl_xor_sync(FULL, bestY, o);
+      const int x2 = __shfl_xor_sync(FULL, bestX, o);
+      const unsigned long long c2 = __shfl_xor_sync(FULL, cells, o);
+      const bool take = (s2 > bestS) || (s2 == bestS && (y2 < bestY || (y2 == bestY && x2 < bestX)));
+      if (take) {
+        bestS = s2;
+        bestY = y2;
+        bestX = x2;
+      }
+      cells += c2;
+    }
+    if (bestS == 0.0f) {  // no positive score anywhere: the first visited cell stands (or nothing was visited)
+      const bool any = ws.firstY >= 0;
+      bestS = any ? 0.0f : -1.0f;
+      bestX = any ? ws.firstX : 0;
+      bestY = any ? ws.firstY : 0;
+    }
+    if (is0) {
+      FillOut o;
+      o.best_score = bestS;
+      o.best_x = bestX;
+      o.best_y = bestY;
+      o.status = status;
+      o.cells = cells;
+      o.dir_shift = 1;
       p.out[ai] = o;
     }
     __syncwarp();
@@ -1033,6 +1558,13 @@ void launch_fill_rf(const FillParams& p, int grid, cudaStream_t stream) {
   else convex_fill_rf_kernel<RAW, true><<<grid, threads, 0, stream>>>(p);
 }
 
+template <bool RAW>
+void launch_fill_rf2(const FillParams& p, int grid, cudaStream_t stream) {
+  const int threads = FILL_WARPS_PER_CTA * 32;
+  if (p.sm_slots) convex_fill_rf2_kernel<RAW, false><<<grid, threads, 0, stream>>>(p);
+  else convex_fill_rf2_kernel<RAW, true><<<grid, threads, 0, stream>>>(p);
+}
+
 template <bool RAW, int NW>
 void launch_fill(const FillParams& p, int grid, cudaStream_t stream) {
   const int threads = (NW == 1 ? FILL_WARPS_PER_CTA : NW) * 32;
@@ -1042,8 +1574,11 @@ void launch_fill(const FillParams& p, int grid, cudaStream_t stream) {
 }  // namespace
 
 // p.sm_slots != nullptr selects the short-lived-CTA instantiation (one problem per warp / team, strips by SM slot)
-cudaError_t launch_convex_fill(const FillParams& p, bool raw, bool team, bool rampfree, int grid, cudaStream_t stream) {
-  if (rampfree) {
+cudaError_t launch_convex_fill(const FillParams& p, bool raw, bool team, int rampfree, int grid, cudaStream_t stream) {
+  if (rampfree == 2) {
+    if (raw) launch_fill_rf2<true>(p, grid, stream);
+    else launch_fill_rf2<false>(p, grid, stream);
+  } else if (rampfree) {
     if (raw) launch_fill_rf<true>(p, grid, stream);
     else launch_fill_rf<false>(p, grid, stream);
   } else if (raw) {
@@ -1063,11 +1598,13 @@ cudaError_t launch_convex_fill_big(const FillParams& p, bool raw, int grid, cuda
   return cudaGetLastError();
 }
 
-int fill_max_ctas_per_sm(bool raw, bool team, bool rampfree) {
+int fill_max_ctas_per_sm(bool raw, bool team, int rampfree) {
   int n = 0;
   const int threads = FILL_WARPS_PER_CTA * 32;
   auto occ = [&](auto kernel) { cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, kernel, threads, 0); };
-  if (rampfree) {
+  if (rampfree == 2) {
+    raw ? occ(convex_fill_rf2_kernel<true, true>) : occ(convex_fill_rf2_kernel<false, true>);
+  } else if (rampfree) {
     raw ? occ(convex_fill_rf_kernel<true, true>) : occ(convex_fill_rf_kernel<false, true>);
   } else if (raw) {
     team ? occ(convex_fill_kernel<true, FILL_WARPS_PER_CTA, true>) : occ(convex_fill_kernel<true, 1, true>);

@@ -34,11 +34,12 @@ struct RowWindow {
   uint32_t w[NW];
 };
 
-__global__ void __launch_bounds__(TB_WARPS_PER_CTA * 32) convex_traceback_kernel(const TraceParams p) {
-  const int slot = blockIdx.x * TB_WARPS_PER_CTA + (threadIdx.x >> 5);
-  const int lane = threadIdx.x & 31;
-  if (slot >= p.n) return;
-  const int i = p.order[slot];  // longest walks first: no straggler warps at the end of the launch
+// The walk of problem i; SH = FillOut::dir_shift, the layout of its direction words (BlockRec), as a constant of the
+// walk's loop.
+template <int SH>
+__device__ __forceinline__ void trace_problem(const TraceParams& p, const int i, const int lane) {
+  constexpr int sh = SH;
+  constexpr unsigned stride = 32u << SH;
   const AlnDesc d = p.desc[i];
   const FillOut f = p.fill[i];
   TraceOut o;
@@ -111,16 +112,15 @@ __global__ void __launch_bounds__(TB_WARPS_PER_CTA * 32) convex_traceback_kernel
         rw.min_c = (int)__fadd_rn((float)rw.off, __fmul_rn(0.1f, wf));
         rw.max_c = (int)__fsub_rn((float)(rw.min_c + rw.len), __fmul_rn(0.1f, wf));
       }
-      // expected step index of the path in row `lane`: two steps per row along the diagonal
-      const int s_here = x - br.base + t;
-      const int s_exp = s_here - 2 * (t - lane);
+      // expected step index of the path in row `lane`: the step of the cell it reaches there along the diagonal
+      const int s_exp = x - (t - lane) - br.base + (lane >> sh);
       int g0 = (s_exp >> 4) - (NW / 2 - 1) - 1;
       g0 = max(0, min(g0, ngroups - NW));
       rw.g0 = g0;
 #pragma unroll
       for (int j = 0; j < NW; ++j) {
         const int g = g0 + j;
-        rw.w[j] = (g < ngroups && lane <= t) ? p.dir[br.word_off + (unsigned long long)g * 32ull + (unsigned)lane] : 0u;
+        rw.w[j] = (g < ngroups && lane <= t) ? p.dir[br.word_off + (unsigned long long)g * stride + (unsigned)lane] : 0u;
       }
     }
     // ---- fast path: a whole run of diagonal moves in one go ----
@@ -132,7 +132,7 @@ __global__ void __launch_bounds__(TB_WARPS_PER_CTA * 32) convex_traceback_kernel
       const int xx = x - (t - lane);
       bool okd = false;
       if (lane <= t && xx >= 0 && xx >= rw.off && (long long)xx < (long long)rw.off + (long long)rw.len) {
-        const int s2 = xx - br.base + lane;
+        const int s2 = xx - br.base + (lane >> sh);
         const int j2 = (s2 >> 4) - rw.g0;
         if ((unsigned)j2 < (unsigned)NW) {
           const uint32_t w2 = j2 == 0 ? rw.w[0] : (j2 == 1 ? rw.w[1] : (j2 == 2 ? rw.w[2] : rw.w[3]));
@@ -186,7 +186,7 @@ __global__ void __launch_bounds__(TB_WARPS_PER_CTA * 32) convex_traceback_kernel
     const int off = __shfl_sync(FULL, rw.off, t);
     const int len = __shfl_sync(FULL, rw.len, t);
     if (x < off || (long long)x >= (long long)off + (long long)len) break;  // STOP: outside the corridor
-    const int s = x - br.base + t;
+    const int s = x - br.base + (t >> sh);
     const int g = s >> 4;
     const int j = g - __shfl_sync(FULL, rw.g0, t);
     uint32_t wd;
@@ -194,7 +194,7 @@ __global__ void __launch_bounds__(TB_WARPS_PER_CTA * 32) convex_traceback_kernel
       const uint32_t mine = j == 0 ? rw.w[0] : (j == 1 ? rw.w[1] : (j == 2 ? rw.w[2] : rw.w[3]));
       wd = __shfl_sync(FULL, mine, t);
     } else {
-      wd = p.dir[br.word_off + (unsigned long long)g * 32ull + (unsigned)t];  // drifted out of the window
+      wd = p.dir[br.word_off + (unsigned long long)g * stride + (unsigned)t];  // drifted out of the window
     }
     const uint32_t code = (wd >> ((s & 15) * 2)) & 3u;
     if (code == DIR_STOP) break;
@@ -286,6 +286,15 @@ __global__ void __launch_bounds__(TB_WARPS_PER_CTA * 32) convex_traceback_kernel
     for (int k = lane; k < n; k += 32) dst[k] = src[k];
   }
   if (lane == 0) p.out[i] = o;
+}
+
+__global__ void __launch_bounds__(TB_WARPS_PER_CTA * 32) convex_traceback_kernel(const TraceParams p) {
+  const int slot = blockIdx.x * TB_WARPS_PER_CTA + (threadIdx.x >> 5);
+  const int lane = threadIdx.x & 31;
+  if (slot >= p.n) return;
+  const int i = p.order[slot];  // longest walks first: no straggler warps at the end of the launch
+  if (p.fill[i].dir_shift) trace_problem<1>(p, i, lane);
+  else trace_problem<0>(p, i, lane);
 }
 
 }  // namespace

@@ -51,8 +51,10 @@ struct alignas(16) AlnDesc {
 };
 
 // One 32-row block of a problem: where its direction words live and how steps map to columns.
-// Cell (x, y) of row y = 32*b + t was computed at step s = x - base + t; its 2-bit code is
-//   dir[word_off + (s >> 4) * 32 + t] >> ((s & 15) * 2).
+// Cell (x, y) of row y = 32*b + t was computed at step s = x - base + (t >> k); its 2-bit code is
+//   dir[word_off + (s >> 4) * (32 << k) + t] >> ((s & 15) * 2),
+// k = FillOut::dir_shift: 0 for the kernels with one row per lane, 1 for the one with two (a lane's two rows share a
+// step; its 16-step group of a 64-row block is one 64-word line, and the second 32-row half starts at word 32).
 struct alignas(16) BlockRec {
   uint64_t word_off;
   int32_t base;
@@ -73,6 +75,7 @@ struct alignas(16) FillOut {
   int32_t best_x, best_y;
   int32_t status;
   unsigned long long cells;
+  int32_t dir_shift;  // layout of the problem's direction words (BlockRec), set by the kernel that filled it
 };
 
 struct alignas(16) TraceOut {

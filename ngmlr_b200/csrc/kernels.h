@@ -17,6 +17,9 @@ constexpr int FILL_CTAS_PER_SM = FILL_CTAS_OVERRIDE;
 #ifndef FILL_TEAM_CTAS_PER_SM
 #define FILL_TEAM_CTAS_PER_SM (FILL_CTAS_OVERRIDE + (FILL_WARPS_OVERRIDE == 4 ? 1 : 0))  // 4-warp teams: 80 registers, 6 CTAs = 24 warps per SM
 #endif
+#ifndef FILL_RF2_CTAS_PER_SM
+#define FILL_RF2_CTAS_PER_SM 4  // the two-row ramp-free kernel: <= 128 registers
+#endif
 constexpr int FILL_SM_SLOTS = 8;   // boundary strips per SM for launches of short-lived CTAs (>= resident CTAs per SM)
 constexpr int FILL_BIG_TEAM = 16;  // warps that pipeline one huge matrix (one CTA per SM)
 
@@ -27,11 +30,12 @@ constexpr int RF_MIN_BLOCK_STEPS = 224;  // steps per 32-row block the ramp-free
 constexpr unsigned long long RF_TEAM_CELLS = 8ull << 20;
 
 // team = all FILL_WARPS_PER_CTA warps of a CTA pipeline one problem; otherwise one warp per problem.
-// rampfree: one warp per problem in the ramp-free row schedule (convex_fill.cu; `team` is ignored).
-cudaError_t launch_convex_fill(const FillParams& p, bool raw, bool team, bool rampfree, int grid, cudaStream_t stream);
+// rampfree 1 / 2: one warp per problem in the ramp-free row schedule with one / two rows per lane (convex_fill.cu;
+// `team` is ignored); 0: the ramped kernels.
+cudaError_t launch_convex_fill(const FillParams& p, bool raw, bool team, int rampfree, int grid, cudaStream_t stream);
 // the same kernel with a FILL_BIG_TEAM-warp team per problem, for the huge matrices of a batch
 cudaError_t launch_convex_fill_big(const FillParams& p, bool raw, int grid, cudaStream_t stream);
-int fill_max_ctas_per_sm(bool raw, bool team, bool rampfree);
+int fill_max_ctas_per_sm(bool raw, bool team, int rampfree);
 // %nsmid of the current device: every %smid is below it (SM ids need not be dense in 0 .. SM count - 1); -1 on error
 int fill_sm_id_bound();
 

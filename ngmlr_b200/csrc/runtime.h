@@ -216,7 +216,9 @@ struct ngmlr_b200_ctx {
   bool team_safe = true;  // every corridor of the batch is monotone with non-empty rows
   int rf_wide = 0;        // problems whose corridor is >= RF_MIN_WIDTH columns wide
   bool rf_fits = true;    // every problem's ramp-free step count fits the kernel's int step numbers
-  unsigned long long rf_problems = 0;  // problems filled by the ramp-free kernel since the context was created
+  unsigned long long rf_problems = 0;  // problems filled by the ramp-free kernels since the context was created
+  unsigned long long rf2_problems = 0; // of those, by the kernel with two rows per lane
+  int rows_per_lane = 2;  // rows per lane of the ramp-free kernel: 1 or 2 (NGMLR_B200_FILL_ROWS_PER_LANE)
   int rf_team = 0;        // problems after the big ones with >= rf_team_cells cells (they lead the order)
   unsigned long long rf_team_cells = nb::RF_TEAM_CELLS;  // NGMLR_B200_RF_TEAM_CELLS
   int fill_schedule = 1;  // 1: ramp-free row schedule where it applies, 2: for every batch, 0: ramped (NGMLR_B200_FILL_SCHEDULE)
@@ -224,7 +226,7 @@ struct ngmlr_b200_ctx {
   nb::PinBuf<unsigned long long> h_win;   // decode_windows: start | arena offset | (sequenceLength, span) pairs
   nb::DevBuf<unsigned long long> d_win;
   int64_t upload_d2h_bytes = 0;
-  int ctas_per_sm[8] = {};  // occupancy of the eight fill-kernel variants (raw x team x ramp-free)
+  int ctas_per_sm[12] = {};  // occupancy of the fill-kernel variants (raw x team x ramped / ramp-free 1 or 2 rows)
   long long debug_arena_words = -1;    // test hook: initial direction-arena size
   nb::PinBuf<uint8_t> h_seq;
   nb::PinBuf<int32_t> h_coff, h_clen, h_order, h_blkbase;
@@ -252,7 +254,7 @@ struct ngmlr_b200_ctx {
   // [4] text_alloc, [5] peaks_alloc, [6] nm_alloc
   nb::DevBuf<unsigned long long> d_counters;
   size_t dir_words_needed = 0;
-  size_t dir_words_rf = 0;  // the same for the ramp-free kernel
+  size_t dir_words_rf = 0;  // the same for the ramp-free kernel (rows_per_lane rows per lane)
   bool ran = false;
   unsigned long long runs_used = 0, dir_used = 0;
   int fill_grid = 0;

@@ -1,13 +1,15 @@
-"""Ramped vs ramp-free row schedule of the convex fill (csrc/convex_fill.cu).
+"""Ramped vs ramp-free row schedule of the convex fill (csrc/convex_fill.cu), the latter with one or two rows per lane.
 
 --cpu (the default) counts, from the bench workload's own corridors, the lane-steps each schedule issues per DP
-cell: the ramped kernel's block_geom arithmetic, and the ramp-free kernel's placement rule restated here (entry at
+cell: the ramped kernel's block_geom arithmetic, and the ramp-free kernels' placement rule restated here (entry at
 a 16-step group boundary, no overlap within a lane, one chunk between a block's last entry and the next block's
-first, the hand-off spacing O_b >= O_{b-1} + RF_RING). No GPU is needed.
+first, the hand-off spacing O_b >= O_{b-1} + RF_RING), for 32-row blocks and for 64-row blocks with two rows per lane.
+A lane-step of the two-row kernel evaluates two cells; "rampfree2" counts cell slots (2 per lane-step) per cell, so the
+three figures compare idle work. No GPU is needed.
 
---gpu runs `bench.py --profile-only` and the full `bench.py` under NGMLR_B200_FILL_SCHEDULE=ramped and =rampfree,
-alternating, and prints the medians and spreads of the fill kernel time and of the headline value, with the card
-name, power limit and SM clock read in the same run.
+--gpu runs `bench.py --profile-only` and the full `bench.py` under NGMLR_B200_FILL_SCHEDULE=ramped, and =rampfree
+with NGMLR_B200_FILL_ROWS_PER_LANE=1 and =2, alternating, and prints the medians and spreads of the fill kernel time
+and of the headline value, with the card name, power limit and SM clock read in the same run.
 
     python scripts/fill_schedule.py --cpu [--reads 300]
     python scripts/fill_schedule.py --gpu --runs 3 --out DIR
@@ -64,15 +66,34 @@ def rf_cols(xlo, xhi, rlen):
     return A, E
 
 
-def rampfree_steps(offs, lens, ref_len):
-    """Steps of the warp under the ramp-free placement (pass 1 of convex_fill_rf_kernel)."""
+def rf2_cols(offs, lens, ref_len, b, H):
+    """Lane t's columns of 64-row block b: its rows 64b + 2t, 64b + 2t + 1 and lane t+1's first row."""
+    xlo0, xhi0, rl0 = spans(offs, lens, ref_len, 2 * b, H)
+    xlo1, xhi1, rl1 = spans(offs, lens, ref_len, 2 * b + 1, H)
+    xlo, xhi, rl = np.concatenate([xlo0, xlo1]), np.concatenate([xhi0, xhi1]), np.concatenate([rl0, rl1])
+    a = np.where(rl > 0, xlo, INT_MAX)
+    e = np.where(rl > 0, xhi, -INT_MAX)
+    aA, aB, eA, eB = a[0::2], a[1::2], e[0::2], e[1::2]
+    a1 = np.append(aA[1:], INT_MAX)
+    e1 = np.append(eA[1:], e.max())
+    amin = np.minimum(np.minimum(aA, aB), a1)
+    A = np.where(amin == INT_MAX, INT_MAX, amin - 1)
+    E = np.maximum(np.maximum(eA, eB), e1)
+    return A, E
+
+
+def rampfree_steps(offs, lens, ref_len, rows=1):
+    """Steps of the warp under the ramp-free placement (pass 1 of convex_fill_rf_kernel / convex_fill_rf2_kernel)."""
     H = len(offs)
     lane = np.arange(32)
     L = np.full(32, -INT_MAX, dtype=np.int64)
     R, O_last = 0, None
-    for b in range((H + 31) // 32):
-        xlo, xhi, rlen = spans(offs, lens, ref_len, b, H)
-        A, E = rf_cols(xlo, xhi, rlen)
+    per = 32 * rows
+    for b in range((H + per - 1) // per):
+        if rows == 1:
+            A, E = rf_cols(*spans(offs, lens, ref_len, b, H))
+        else:
+            A, E = rf2_cols(offs, lens, ref_len, b, H)
         has = A != INT_MAX
         frm = np.maximum(L, R)
         need = np.where(has, ((frm + 15) // 16) * 16 - lane - A, -INT_MAX)
@@ -95,7 +116,7 @@ def cpu(args):
     contig = 10_000_000
     genome = synth.random_genome(5 * contig, 1)
     reads, ivs = synth.simulate_reads(args.reads, genome, contig, 3, **cfg)
-    cells = ramp = rf = 0
+    cells = ramp = rf = rf2 = 0
     widths = []
     for iv in ivs:
         p = iv.problem(genome, reads)
@@ -106,6 +127,7 @@ def cpu(args):
         widths.append(int(lens.max()))
         ramp += 32 * ramped_steps(offs, lens, ref_len)
         rf += 32 * rampfree_steps(offs, lens, ref_len)
+        rf2 += 64 * rampfree_steps(offs, lens, ref_len, rows=2)
     w = np.array(widths)
     out = {
         "problems": len(ivs),
@@ -113,6 +135,7 @@ def cpu(args):
         "lane_steps_per_cell": {
             "ramped": round(ramp / cells, 4),
             "rampfree": round(rf / cells, 4),
+            "rampfree2": round(rf2 / cells, 4),
         },
     }
     print(json.dumps(out, indent=1))
@@ -124,22 +147,26 @@ def smi():
     return r.stdout.strip().splitlines()[0] if r.returncode == 0 and r.stdout.strip() else "nvidia-smi unavailable"
 
 
-def bench(schedule, extra, steps, warmup):
-    env = dict(os.environ, NGMLR_B200_FILL_SCHEDULE=schedule)
+SETTINGS = {"ramped": ("ramped", "1"), "rampfree-rows1": ("rampfree", "1"), "rampfree-rows2": ("rampfree", "2")}
+
+
+def bench(setting, extra, steps, warmup):
+    schedule, rows = SETTINGS[setting]
+    env = dict(os.environ, NGMLR_B200_FILL_SCHEDULE=schedule, NGMLR_B200_FILL_ROWS_PER_LANE=rows)
     cmd = [sys.executable, os.path.join(ROOT, "bench.py"), "--gpus", "1", "--steps", str(steps),
            "--warmup", str(warmup)] + extra
     r = subprocess.run(cmd, env=env, capture_output=True, text=True, cwd=ROOT)
     lines = [l for l in r.stdout.splitlines() if l.startswith("{")]
     if r.returncode != 0 or not lines:
-        raise SystemExit(f"bench.py failed ({schedule} {extra}):\n{r.stdout[-3000:]}\n{r.stderr[-3000:]}")
+        raise SystemExit(f"bench.py failed ({setting} {extra}):\n{r.stdout[-3000:]}\n{r.stderr[-3000:]}")
     return json.loads(lines[-1])
 
 
 def gpu(args):
     print("card:", smi())
-    res = {"ramped": {"prof": [], "full": []}, "rampfree": {"prof": [], "full": []}}
+    res = {k: {"prof": [], "full": []} for k in SETTINGS}
     for i in range(args.runs):
-        for sched in ("ramped", "rampfree"):
+        for sched in SETTINGS:
             prof = bench(sched, ["--profile-only"], args.steps, args.warmup)
             full = bench(sched, [], args.steps, args.warmup)
             res[sched]["prof"].append(prof)
@@ -150,12 +177,14 @@ def gpu(args):
     for sched, r in res.items():
         fill = np.array([x["kernel_ms_per_step"]["fill"] for x in r["full"]])
         val = np.array([x["value"] for x in r["full"]])
+        pfill = np.array([x["fill_ms"] for x in r["prof"]])
         summary[sched] = {"fill_ms_median": float(np.median(fill)), "fill_ms_spread": float(fill.max() - fill.min()),
                           "value_median": float(np.median(val)), "value_spread": float(val.max() - val.min()),
-                          "fill_ms": fill.tolist(), "value": val.tolist()}
-    a, b = summary["ramped"], summary["rampfree"]
-    summary["fill_change"] = b["fill_ms_median"] / a["fill_ms_median"] - 1.0
-    summary["value_change"] = b["value_median"] / a["value_median"] - 1.0
+                          "solo_fill_ms_median": float(np.median(pfill)), "fill_ms": fill.tolist(),
+                          "value": val.tolist()}
+    for a, b in (("ramped", "rampfree-rows1"), ("rampfree-rows1", "rampfree-rows2")):
+        summary[f"fill_change {a} -> {b}"] = summary[b]["fill_ms_median"] / summary[a]["fill_ms_median"] - 1.0
+        summary[f"value_change {a} -> {b}"] = summary[b]["value_median"] / summary[a]["value_median"] - 1.0
     print(json.dumps(summary, indent=1))
     if args.out:
         os.makedirs(args.out, exist_ok=True)
@@ -166,7 +195,7 @@ def gpu(args):
 def main():
     ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
     ap.add_argument("--cpu", action="store_true", help="lane-steps per cell from the workload geometry (default)")
-    ap.add_argument("--gpu", action="store_true", help="A/B of both schedules with bench.py")
+    ap.add_argument("--gpu", action="store_true", help="A/B of the schedules with bench.py")
     ap.add_argument("--reads", type=int, default=300)
     ap.add_argument("--runs", type=int, default=3)
     ap.add_argument("--steps", type=int, default=5)
