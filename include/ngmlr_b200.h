@@ -119,6 +119,11 @@ int ngmlr_b200_set_fill_ctas_per_sm(ngmlr_b200_ctx* ctx, int ctas_per_sm);
  * NGMLR_B200_SMALL_BATCH_BIG_TEAMS=0). Default on. No reference counterpart. Results do not depend on it. */
 int ngmlr_b200_set_small_batch_teams(ngmlr_b200_ctx* ctx, int on);
 
+/* Frees the device and pinned host arenas the context's convex batches grew (they grow again on the next batch).
+ * The results of the last batch become invalid. The C++ plugin calls it when a batch ran out of memory, before it
+ * splits the batch and retries the halves. No reference counterpart. */
+int ngmlr_b200_release_arenas(ngmlr_b200_ctx* ctx);
+
 /* ---- convex banded alignment: IAlignment::SingleAlign(mode, CorridorLine*, ...) batched -------
  * Replaces ConvexAlignFast::SingleAlign (src/ConvexAlignFast.cpp:452-559) for n independent
  * problems. Problem i: refs[i]/qrys[i] are the reference window and read part (need not be

@@ -55,7 +55,7 @@ class Interval(C.Structure):
 C_API_SYMBOLS = (
     "ngmlr_b200_abi_version", "ngmlr_b200_device_count", "ngmlr_b200_create", "ngmlr_b200_destroy",
     "ngmlr_b200_last_error", "ngmlr_b200_set_stream", "ngmlr_b200_get_stream",
-    "ngmlr_b200_set_fill_ctas_per_sm", "ngmlr_b200_set_small_batch_teams",
+    "ngmlr_b200_set_fill_ctas_per_sm", "ngmlr_b200_set_small_batch_teams", "ngmlr_b200_release_arenas",
     "ngmlr_b200_convex_align_batch", "ngmlr_b200_convex_upload", "ngmlr_b200_convex_run",
     "ngmlr_b200_convex_fetch", "ngmlr_b200_convex_stats", "ngmlr_b200_convex_debug_directions",
     "ngmlr_b200_sw_score_batch", "ngmlr_b200_cs_set_index", "ngmlr_b200_cs_search_batch",
@@ -106,6 +106,10 @@ def load():
     lib.ngmlr_b200_set_fill_ctas_per_sm.argtypes = [vp, C.c_int]
     lib.ngmlr_b200_set_small_batch_teams.argtypes = [vp, C.c_int]
     lib.ngmlr_b200_debug_set_arena_words.argtypes = [vp, C.c_longlong]
+    lib.ngmlr_b200_debug_set_arena_cap.argtypes = [vp, C.c_longlong]
+    lib.ngmlr_b200_debug_arena_bytes.argtypes = [vp]
+    lib.ngmlr_b200_debug_arena_bytes.restype = C.c_longlong
+    lib.ngmlr_b200_release_arenas.argtypes = [vp]
     lib.ngmlr_b200_debug_rampfree_problems.argtypes = [vp]
     lib.ngmlr_b200_debug_rampfree_problems.restype = C.c_longlong
     lib.ngmlr_b200_debug_rampfree2_problems.argtypes = [vp]
@@ -169,5 +173,7 @@ def load():
                                                 C.c_char_p, C.c_char_p, C.c_int]
     lib.ngmlr_b200_sw_last_kernel_ms.argtypes = [vp]
     lib.ngmlr_b200_sw_last_kernel_ms.restype = C.c_float
+    lib.ngmlr_b200_plugin_context.argtypes = [vp]
+    lib.ngmlr_b200_plugin_context.restype = vp
     _lib = lib
     return lib

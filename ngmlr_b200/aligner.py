@@ -570,6 +570,19 @@ class B200Aligner:
         """Test hook: initial size of the direction arena (-1 = the host's estimate)."""
         self.lib.ngmlr_b200_debug_set_arena_words(self.h, int(words))
 
+    def debug_set_arena_cap(self, nbytes):
+        """Test hook: the device arenas of convex batches may hold at most `nbytes` bytes (-1 = no cap); a batch that
+        needs more fails with "out of memory" as on a full device."""
+        self.lib.ngmlr_b200_debug_set_arena_cap(self.h, int(nbytes))
+
+    def debug_arena_bytes(self):
+        """Test hook: bytes the device arenas of convex batches hold now."""
+        return int(self.lib.ngmlr_b200_debug_arena_bytes(self.h))
+
+    def release_arenas(self):
+        """Free the arenas the convex batches grew (see ngmlr_b200_release_arenas)."""
+        self._check(self.lib.ngmlr_b200_release_arenas(self.h))
+
     def debug_rampfree_problems(self):
         """Test hook: problems filled by the ramp-free fill kernels since the context was created."""
         return int(self.lib.ngmlr_b200_debug_rampfree_problems(self.h))

@@ -143,6 +143,7 @@ int ngmlr_b200_create(int gpu_id, const ngmlr_b200_scoring* s, ngmlr_b200_ctx** 
   if (const char* e = getenv("NGMLR_B200_RF_TEAM_CELLS")) ctx->rf_team_cells = strtoull(e, nullptr, 10);
   if (const char* e = getenv("NGMLR_B200_FILL_CTAS_PER_SM")) ctx->fill_ctas_cap = std::max(0, atoi(e));
   if (const char* e = getenv("NGMLR_B200_NO_CORRIDOR_PACKING")) ctx->no_corridor_packing = atoi(e);
+  if (const char* e = getenv("NGMLR_B200_DEBUG_ARENA_CAP")) ctx->debug_arena_cap = std::max(-1LL, atoll(e));
   *out = ctx;
   return 0;
 }
@@ -197,6 +198,44 @@ void* ngmlr_b200_get_stream(ngmlr_b200_ctx* ctx) { return ctx ? (void*)ctx->stre
 int ngmlr_b200_debug_set_arena_words(ngmlr_b200_ctx* ctx, long long words) {
   if (!ctx) return -1;
   ctx->debug_arena_words = words;
+  return 0;
+}
+
+// Test hooks: the device arenas of convex batches may hold at most `bytes` bytes (-1 = no cap; NGMLR_B200_DEBUG_ARENA_CAP
+// sets it at creation), and what they hold now. A batch that needs more than the cap fails with "out of memory", as on
+// a full device, deterministically and without touching the driver's limits.
+int ngmlr_b200_debug_set_arena_cap(ngmlr_b200_ctx* ctx, long long bytes) {
+  if (!ctx) return -1;
+  ctx->debug_arena_cap = bytes < 0 ? -1 : bytes;
+  return 0;
+}
+
+long long ngmlr_b200_debug_arena_bytes(ngmlr_b200_ctx* ctx) { return ctx ? (long long)ctx->arena_bytes : -1; }
+
+int ngmlr_b200_release_arenas(ngmlr_b200_ctx* ctx) {
+  if (!ctx) return -1;
+  CU(cudaSetDevice(ctx->device));
+  nb_stream_sync(ctx, ctx->stream);
+  ctx->arena_release(ctx->d_seq); ctx->arena_release(ctx->d_coff); ctx->arena_release(ctx->d_clen);
+  ctx->arena_release(ctx->d_order); ctx->arena_release(ctx->d_blkbase); ctx->arena_release(ctx->d_delta);
+  ctx->arena_release(ctx->d_desc); ctx->arena_release(ctx->d_blocks); ctx->arena_release(ctx->d_dir);
+  ctx->arena_release(ctx->d_bnd); ctx->arena_release(ctx->d_fill); ctx->arena_release(ctx->d_scratch);
+  ctx->arena_release(ctx->d_trace); ctx->arena_release(ctx->d_runs); ctx->arena_release(ctx->d_counters);
+  ctx->arena_release(ctx->d_aux); ctx->arena_release(ctx->d_sm_slots); ctx->arena_release(ctx->d_textout);
+  ctx->arena_release(ctx->d_text); ctx->arena_release(ctx->d_peaks); ctx->arena_release(ctx->d_nm);
+  ctx->sm_slots_zeroed = false;
+  ctx->h_seq.release(); ctx->h_coff.release(); ctx->h_clen.release(); ctx->h_order.release(); ctx->h_blkbase.release();
+  ctx->h_delta.release(); ctx->h_desc.release(); ctx->h_fill.release(); ctx->h_trace.release(); ctx->h_runs.release();
+  ctx->h_counters.release(); ctx->h_aux.release(); ctx->h_textout.release();
+  for (int s = 0; s < TEXT_SLOTS; ++s) {
+    ctx->h_text[s].release();
+    ctx->h_peaks[s].release();
+    ctx->h_nm[s].release();
+  }
+  ctx->n = 0;
+  ctx->ran = false;
+  // a cudaMalloc that failed stays the thread's last error: the launch checks of the next batch must not see it
+  cudaGetLastError();
   return 0;
 }
 

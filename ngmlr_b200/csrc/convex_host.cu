@@ -238,17 +238,17 @@ int convex_upload_spec(ngmlr_b200_ctx* ctx, const UploadSpec& sp) {
   const double t_pack1 = now_ms();
   // ---- device arenas + H2D ----
   cudaStream_t st = ctx->stream;
-  CU(ctx->d_seq.reserve(so + 64));
-  CU(ctx->d_coff.reserve(rows + 32));
-  CU(ctx->d_clen.reserve(rows + 32));
-  CU(ctx->d_desc.reserve(n));
-  CU(ctx->d_order.reserve(n));
-  CU(ctx->d_blocks.reserve(bo + 1));
-  CU(ctx->d_fill.reserve(n));
-  CU(ctx->d_trace.reserve(n));
-  CU(ctx->d_scratch.reserve(tb_ints + 32));
-  CU(ctx->d_runs.reserve(tb_ints / 4 + 4096));
-  CU(ctx->d_counters.reserve(8));
+  CU(ctx->arena_reserve(ctx->d_seq, so + 64));
+  CU(ctx->arena_reserve(ctx->d_coff, rows + 32));
+  CU(ctx->arena_reserve(ctx->d_clen, rows + 32));
+  CU(ctx->arena_reserve(ctx->d_desc, n));
+  CU(ctx->arena_reserve(ctx->d_order, n));
+  CU(ctx->arena_reserve(ctx->d_blocks, bo + 1));
+  CU(ctx->arena_reserve(ctx->d_fill, n));
+  CU(ctx->arena_reserve(ctx->d_trace, n));
+  CU(ctx->arena_reserve(ctx->d_scratch, tb_ints + 32));
+  CU(ctx->arena_reserve(ctx->d_runs, tb_ints / 4 + 4096));
+  CU(ctx->arena_reserve(ctx->d_counters, 8));
   CU(ctx->h_counters.reserve(8));
   CU(ctx->h_fill.reserve(n));
   CU(ctx->h_trace.reserve(n));
@@ -268,7 +268,7 @@ int convex_upload_spec(ngmlr_b200_ctx* ctx, const UploadSpec& sp) {
     const size_t nn = (size_t)n;
     const size_t aux_bytes = nn * (3 * 8 + 6 * 4 + 1) + 64;
     CU(ctx->h_aux.reserve(aux_bytes));
-    CU(ctx->d_aux.reserve(aux_bytes));
+    CU(ctx->arena_reserve(ctx->d_aux, aux_bytes));
     unsigned char* ha = ctx->h_aux.p;
     uint64_t* a_win = reinterpret_cast<uint64_t*>(ha);
     uint64_t* a_roff = a_win + nn;
@@ -345,8 +345,8 @@ int convex_upload_spec(ngmlr_b200_ctx* ctx, const UploadSpec& sp) {
         raw_rows += (size_t)qry_lens[i];
         ++raw_problems;
       }
-    CU(ctx->d_delta.reserve(rows + 32));
-    CU(ctx->d_blkbase.reserve(bo + 1));
+    CU(ctx->arena_reserve(ctx->d_delta, rows + 32));
+    CU(ctx->arena_reserve(ctx->d_blkbase, bo + 1));
     if (rows) {
       CU(cudaMemcpyAsync(ctx->d_delta.p, ctx->h_delta.p, rows, cudaMemcpyHostToDevice, st));
       CU(cudaMemcpyAsync(ctx->d_blkbase.p, ctx->h_blkbase.p, bo * sizeof(int32_t), cudaMemcpyHostToDevice, st));
@@ -365,8 +365,8 @@ int convex_upload_spec(ngmlr_b200_ctx* ctx, const UploadSpec& sp) {
     }
     h2d += rows + bo * 4 + raw_rows * 8;
   } else {
-    CU(ctx->d_delta.reserve(32));
-    CU(ctx->d_blkbase.reserve(bo + 1));
+    CU(ctx->arena_reserve(ctx->d_delta, 32));
+    CU(ctx->arena_reserve(ctx->d_blkbase, bo + 1));
   }
   CU(cudaMemcpyAsync(ctx->d_desc.p, ctx->h_desc.p, (size_t)n * sizeof(AlnDesc), cudaMemcpyHostToDevice, st));
   CU(cudaMemcpyAsync(ctx->d_order.p, ctx->h_order.p, (size_t)n * sizeof(int32_t), cudaMemcpyHostToDevice, st));
@@ -463,7 +463,7 @@ int ngmlr_b200_convex_run(ngmlr_b200_ctx* ctx) {
   const size_t strips = persistent ? (size_t)grid : (size_t)ctx->sm_ids * FILL_SM_SLOTS;
   const size_t warps = strips * (team ? 1 : FILL_WARPS_PER_CTA);  // a team shares one strip
   if (!persistent) {
-    CU(ctx->d_sm_slots.reserve((size_t)ctx->sm_ids));
+    CU(ctx->arena_reserve(ctx->d_sm_slots, (size_t)ctx->sm_ids));
     if (!ctx->sm_slots_zeroed) {
       CU(cudaMemsetAsync(ctx->d_sm_slots.p, 0, (size_t)ctx->sm_ids * sizeof(unsigned int), st));
       ctx->sm_slots_zeroed = true;
@@ -482,12 +482,12 @@ int ngmlr_b200_convex_run(ngmlr_b200_ctx* ctx) {
   // ramped 4-warp teams beside the one-warp launch, one CTA per SM at most
   const int n_team = rampfree && ctx->team_safe && ctx->force_team != 0 ? std::min(ctx->rf_team, n - n_big) : 0;
   const int team_grid = std::min(n_team, ctx->num_sms);
-  CU(ctx->d_bnd.reserve((warps + (size_t)big_grid + (size_t)team_grid) * bnd_stride));
+  CU(ctx->arena_reserve(ctx->d_bnd, (warps + (size_t)big_grid + (size_t)team_grid) * bnd_stride));
   size_t& words_needed = rampfree ? ctx->dir_words_rf : ctx->dir_words_needed;
   size_t dir_words = std::max(words_needed, (size_t)4096);
   if (ctx->debug_arena_words >= 0) {  // force the overflow -> grow -> re-run path (tests)
     dir_words = (size_t)ctx->debug_arena_words;
-    ctx->d_dir.release();
+    ctx->arena_release(ctx->d_dir);
   }
   size_t runs_cap = ctx->d_runs.cap;
   const bool dev_text = ctx->text_mode != 0;
@@ -496,14 +496,14 @@ int ngmlr_b200_convex_run(ngmlr_b200_ctx* ctx) {
     text_cap = std::max(ctx->d_text.cap, ctx->debug_arena_words >= 0 ? (size_t)256 : ctx->text_cap_hint);
     peaks_cap = std::max(ctx->d_peaks.cap, (size_t)n * 4 + 1024);
     nm_cap = ctx->want_nm ? std::max(ctx->d_nm.cap, (size_t)3 * (ctx->tb_ints + 64)) : 0;
-    CU(ctx->d_textout.reserve(n));
+    CU(ctx->arena_reserve(ctx->d_textout, n));
     CU(ctx->h_textout.reserve(n));
   }
   bool need_fill = true;
 
   for (int attempt = 0; attempt < 24; ++attempt) {
-    CU(ctx->d_dir.reserve(dir_words));
-    CU(ctx->d_runs.reserve(runs_cap));
+    CU(ctx->arena_reserve(ctx->d_dir, dir_words));
+    CU(ctx->arena_reserve(ctx->d_runs, runs_cap));
     if (need_fill) CU(cudaMemsetAsync(ctx->d_counters.p, 0, 8 * sizeof(unsigned long long), st));
     else CU(cudaMemsetAsync(ctx->d_counters.p + 4, 0, 4 * sizeof(unsigned long long), st));
     if (need_fill) {
@@ -595,9 +595,9 @@ int ngmlr_b200_convex_run(ngmlr_b200_ctx* ctx) {
       ctx->stats.traceback_launches++;
     }
     if (dev_text) {
-      CU(ctx->d_text.reserve(text_cap));
-      CU(ctx->d_peaks.reserve(peaks_cap));
-      if (nm_cap) CU(ctx->d_nm.reserve(nm_cap));
+      CU(ctx->arena_reserve(ctx->d_text, text_cap));
+      CU(ctx->arena_reserve(ctx->d_peaks, peaks_cap));
+      if (nm_cap) CU(ctx->arena_reserve(ctx->d_nm, nm_cap));
       TextParams xp;
       xp.seq = ctx->d_seq.p;
       xp.desc = ctx->d_desc.p;

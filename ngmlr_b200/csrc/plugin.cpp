@@ -45,6 +45,8 @@ struct PluginStats {
   std::atomic<long long> score_calls{0}, score_batches{0}, score_pairs{0}, score_batch_us{0};
   // time the calling threads spent blocked inside the batched calls (summed over threads), microseconds
   std::atomic<long long> align_wait_us{0}, score_wait_us{0};
+  // batched SingleAlign / BatchAlign launches that ran out of memory and were split in halves
+  std::atomic<long long> align_oom_splits{0};
   const std::chrono::steady_clock::time_point t_start = std::chrono::steady_clock::now();
   // phases of the batched SingleAlign launches, microseconds (from ngmlr_b200_convex_stats + the copy back)
   std::atomic<long long> us_pack{0}, us_h2d{0}, us_run{0}, us_fill{0}, us_trace{0}, us_d2h{0}, us_text{0}, us_copy{0};
@@ -70,6 +72,8 @@ struct PluginStats {
             "%.2f), D2H %.2f, CIGAR/MD/nmPerPosition text %.2f, copy into the callers' Align %.2f\n",
             1e-3 * us_pack / nb, 1e-3 * us_h2d / nb, 1e-3 * us_run / nb, 1e-3 * us_fill / nb, 1e-3 * us_trace / nb,
             1e-3 * us_d2h / nb, 1e-3 * us_text / nb, 1e-3 * us_copy / nb);
+    if (align_oom_splits)
+      fprintf(stderr, "[ngmlr_b200] alignment batches split after running out of memory: %lld\n", align_oom_splits.load());
   }
 } g_stats;
 
@@ -307,36 +311,65 @@ class B200Alignment : public IAlignment {
       rets[i] = -1;
       if (threw_out) threw_out[i] = false;
     }
-    if (m > 0) {
-      int rc = ngmlr_b200_convex_align_batch(ctx(), m, krefs_.data(), krl_.data(), kqrys_.data(), kql_.data(),
-                                             off_.data(), len_.data(), row_start_.data(), kqs_.data(),
-                                             kqe_.data(), res_.data());
-      if (rc != 0) {
-        // Device memory exhausted by the direction matrix is the reference's "matrix too large": -1
-        // per problem instead of an exception that would end the whole run.
-        const char* e = ngmlr_b200_last_error(ctx_);
-        if (e && strstr(e, "out of memory")) return;
+    std::vector<char> threw_j((size_t)std::max(m, 1), 0);
+    if (m > 0) align_range(0, m, results, rets, threw_j, false);
+    bool threw = false;
+    for (int j = 0; j < m; ++j)
+      if (threw_j[j]) {
+        threw = true;
+        if (threw_out) threw_out[keep_[j]] = true;
+      }
+    if (threw && n == 1 && !threw_out) throw 1;  // caller wraps SingleAlign in try/catch(...) -> unmapped
+  }
+
+ private:
+  // The kept problems [j0, j1) through one batched call, their results copied into the callers' Align records.
+  // A batch that runs out of memory (device arenas or pinned staging) runs again on released arenas (`fresh`), and
+  // if it still does not fit, as two halves one after the other: n independent SingleAlign calls would each have
+  // fitted where the batch did not. Only a problem that runs out of memory alone on released arenas fails, with
+  // Score -1 -- the reference's "matrix too large".
+  void align_range(int j0, int j1, Align* const* results, int* rets, std::vector<char>& threw_j, bool fresh) {
+    const int m = j1 - j0;
+    std::vector<int64_t> rs((size_t)m + 1);
+    for (int k = 0; k <= m; ++k) rs[k] = row_start_[j0 + k] - row_start_[j0];
+    const int rc = ngmlr_b200_convex_align_batch(ctx(), m, krefs_.data() + j0, krl_.data() + j0, kqrys_.data() + j0,
+                                                 kql_.data() + j0, off_.data() + row_start_[j0],
+                                                 len_.data() + row_start_[j0], rs.data(), kqs_.data() + j0,
+                                                 kqe_.data() + j0, res_.data());
+    if (rc != 0) {
+      const char* e = ngmlr_b200_last_error(ctx_);
+      if (!(e && strstr(e, "out of memory"))) {
         error_ = e ? e : "ngmlr_b200: batched alignment failed";
         throw error_.c_str();
       }
-    }
-    if (m > 0) {
-      ngmlr_b200_batch_stats bs;
-      if (ngmlr_b200_convex_stats(ctx_, &bs) == 0) {
-        g_stats.us_pack += (long long)(1e3 * bs.host_pack_ms);
-        g_stats.us_h2d += (long long)(1e3 * bs.host_h2d_ms);
-        g_stats.us_run += (long long)(1e3 * bs.host_run_ms);
-        g_stats.us_fill += (long long)(1e3 * bs.fill_ms);
-        g_stats.us_trace += (long long)(1e3 * bs.traceback_ms);
-        g_stats.us_d2h += (long long)(1e3 * bs.host_d2h_ms);
-        g_stats.us_text += (long long)(1e3 * bs.host_text_ms);
+      ngmlr_b200_release_arenas(ctx_);
+      if (!fresh) {
+        align_range(j0, j1, results, rets, threw_j, true);
+        return;
       }
+      if (m == 1) return;  // Score -1, ret -1 (set by align_many)
+      g_stats.align_oom_splits++;
+      const int mid = j0 + m / 2;
+      align_range(j0, mid, results, rets, threw_j, true);
+      align_range(mid, j1, results, rets, threw_j, false);
+      return;
     }
+    ngmlr_b200_batch_stats bs;
+    if (ngmlr_b200_convex_stats(ctx_, &bs) == 0) {
+      g_stats.us_pack += (long long)(1e3 * bs.host_pack_ms);
+      g_stats.us_h2d += (long long)(1e3 * bs.host_h2d_ms);
+      g_stats.us_run += (long long)(1e3 * bs.host_run_ms);
+      g_stats.us_fill += (long long)(1e3 * bs.fill_ms);
+      g_stats.us_trace += (long long)(1e3 * bs.traceback_ms);
+      g_stats.us_d2h += (long long)(1e3 * bs.host_d2h_ms);
+      g_stats.us_text += (long long)(1e3 * bs.host_text_ms);
+    }
+    // the results point into the context's arenas: copy them out before the next batch call
     const auto t_copy0 = std::chrono::steady_clock::now();
-    std::vector<char> threw_j((size_t)std::max(m, 1), 0);
-    plugin_parallel_for(m, 16, [&](int j) {
+    plugin_parallel_for(m, 16, [&](int jj) {
+      const int j = j0 + jj;
       const int i = keep_[j];
-      const ngmlr_b200_align_result& r = res_[j];
+      const ngmlr_b200_align_result& r = res_[jj];
       Align& a = *results[i];
       if (a.pBuffer2) a.pBuffer2[0] = '\0';  // (:469)
       if (r.threw) {
@@ -385,17 +418,9 @@ class B200Alignment : public IAlignment {
       a.svType = r.sv_type;
       rets[i] = r.ret;
     });
-    bool threw = false;
-    for (int j = 0; j < m; ++j)
-      if (threw_j[j]) {
-        threw = true;
-        if (threw_out) threw_out[keep_[j]] = true;
-      }
     g_stats.us_copy += std::chrono::duration_cast<std::chrono::microseconds>(std::chrono::steady_clock::now() - t_copy0).count();
-    if (threw && n == 1 && !threw_out) throw 1;  // caller wraps SingleAlign in try/catch(...) -> unmapped
   }
 
- private:
   int gpu_id_ = 0;
   bool device_ok_ = false;
   ngmlr_b200_scoring scoring_;
@@ -698,6 +723,19 @@ void SetAlignmentScoring(float match, float mismatch, float gapOpen, float gapEx
 }
 
 int ngmlr_b200_plugin_cookie(void) { return 0x10201130; }  // cCookie, src/IAlignment.h:193
+
+// Test / diagnostic aid: the device context an object made by CreateAlignment runs its direct calls on (created
+// here if it has none yet), so that FFI callers can read its last error and batch statistics or set its test hooks.
+// NULL for any other object or when no context can be made.
+ngmlr_b200_ctx* ngmlr_b200_plugin_context(IAlignment* aligner) {
+  B200Alignment* a = dynamic_cast<B200Alignment*>(aligner);
+  if (!a) return nullptr;
+  try {
+    return a->ctx();
+  } catch (...) {
+    return nullptr;
+  }
+}
 
 // Benchmark / test aid for FFI callers that cannot build C++ objects (bench.py): n SingleAlign problems
 // given as flat arrays are turned into what ngmlr itself would hold -- caller-allocated `Align` records

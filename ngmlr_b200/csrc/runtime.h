@@ -28,14 +28,18 @@ template <typename T>
 struct DevBuf {
   T* p = nullptr;
   size_t cap = 0;  // elements
+  // the capacity reserve(n) grows to (n > cap)
+  size_t grown(size_t n) const { return borrowed ? n : std::max(n, cap + cap / 2); }
+  // bytes of device memory the buffer owns
+  size_t owned_bytes() const { return borrowed ? 0 : cap * sizeof(T); }
   cudaError_t reserve(size_t n, bool keep = false, cudaStream_t st = 0) {
     if (n <= cap) return cudaSuccess;
+    const size_t want = grown(n);
     if (borrowed) {  // never grow (or free) somebody else's memory: start an own buffer
       p = nullptr;
       cap = 0;
       borrowed = false;
     }
-    size_t want = std::max(n, cap + cap / 2);
     T* q = nullptr;
     cudaError_t e = cudaMalloc(&q, want * sizeof(T));
     if (e != cudaSuccess) return e;
@@ -228,6 +232,26 @@ struct ngmlr_b200_ctx {
   int64_t upload_d2h_bytes = 0;
   int ctas_per_sm[12] = {};  // occupancy of the fill-kernel variants (raw x team x ramped / ramp-free 1 or 2 rows)
   long long debug_arena_words = -1;    // test hook: initial direction-arena size
+  // Test hook (ngmlr_b200_debug_set_arena_cap, NGMLR_B200_DEBUG_ARENA_CAP): the device arenas of convex batches may
+  // hold at most this many bytes (-1: no cap). A reservation beyond it fails the way cudaMalloc does when the device
+  // is full ("out of memory"), without asking the driver for anything.
+  long long debug_arena_cap = -1;
+  size_t arena_bytes = 0;  // bytes the convex-batch device arenas hold (all of them reserve through arena_reserve)
+  template <typename T>
+  cudaError_t arena_reserve(nb::DevBuf<T>& b, size_t n) {
+    if (n <= b.cap) return cudaSuccess;
+    const size_t held = b.owned_bytes();
+    if (debug_arena_cap >= 0 && arena_bytes - held + b.grown(n) * sizeof(T) > (size_t)debug_arena_cap)
+      return cudaErrorMemoryAllocation;
+    const cudaError_t e = b.reserve(n);
+    if (e == cudaSuccess) arena_bytes += b.owned_bytes() - held;
+    return e;
+  }
+  template <typename T>
+  void arena_release(nb::DevBuf<T>& b) {
+    arena_bytes -= b.owned_bytes();
+    b.release();
+  }
   nb::PinBuf<uint8_t> h_seq;
   nb::PinBuf<int32_t> h_coff, h_clen, h_order, h_blkbase;
   nb::PinBuf<int8_t> h_delta;

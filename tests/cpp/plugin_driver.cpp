@@ -3,13 +3,16 @@
 // CorridorLine[], BatchAlign with NgmlrB200BatchAlignArgs, BatchScore, SingleScore) with
 // caller-allocated Align buffers (src/AlignmentBuffer.cpp:271-278). Problems are read from a
 // simple text file written by tests/test_gpu_plugin.py, results are printed one line per problem
-// for comparison with the oracle.
+// for comparison with the oracle. An optional third argument runs the SingleAlign calls from that many threads at
+// once (with NGMLR_B200_BATCH_WINDOW_US set the cross-thread batcher then serves several of them per launch).
 #include <dlfcn.h>
+#include <stdint.h>
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
 
 #include <string>
+#include <thread>
 #include <vector>
 
 #include "ngmlr_b200_ialignment.h"
@@ -35,6 +38,23 @@ static void print_align(const char* tag, int i, int ret, const Align& a) {
          a.lastPosition.refPosition, a.lastPosition.readPosition, a.pBuffer1, a.pBuffer2);
 }
 
+// nmPerPosition (the triples ngmlr's SV logic reads): count and FNV-1a over (refPosition, readPosition, nm) as
+// little-endian int32s, on a line of its own so that the lines above keep their format. The Align record carries no
+// count, so alloc_align fills the array with a pattern no triple can take; the written entries are the ones before it.
+static const int32_t kNmUnset = INT32_MIN;
+static void print_nm(const char* tag, int i, int ret, const Align& a) {
+  if (ret < 0) return;
+  int count = 0;
+  uint32_t h = 2166136261u;
+  while (a.nmPerPosition && count < a.nmPerPostionLength && a.nmPerPosition[count].nm != kNmUnset) {
+    const PositionNM& p = a.nmPerPosition[count++];
+    const int32_t v[3] = {p.refPosition, p.readPosition, p.nm};
+    const unsigned char* b = reinterpret_cast<const unsigned char*>(v);
+    for (int x = 0; x < 12; ++x) h = (h ^ b[x]) * 16777619u;
+  }
+  printf("nm %s %d count=%d fnv=%u\n", tag, i, count, h);
+}
+
 static void alloc_align(Align& a, size_t readLength) {
   a.maxBufferLength = (int)readLength * 4 + 8;
   a.maxMdBufferLength = (int)readLength * 4 + 8;
@@ -43,6 +63,8 @@ static void alloc_align(Align& a, size_t readLength) {
   a.pBuffer1[0] = a.pBuffer2[0] = '\0';
   a.nmPerPostionLength = ((int)readLength + 1) * 2;
   a.nmPerPosition = new PositionNM[a.nmPerPostionLength];
+  for (int k = 0; k < a.nmPerPostionLength; ++k) a.nmPerPosition[k].refPosition = a.nmPerPosition[k].readPosition =
+      a.nmPerPosition[k].nm = kNmUnset;
 }
 
 int main(int argc, char** argv) {
@@ -74,27 +96,41 @@ int main(int argc, char** argv) {
   fclose(f);
 
   printf("batchsize %d %d\n", al->GetScoreBatchSize(), al->GetAlignBatchSize());
-  // 1) one blocking SingleAlign per problem, as computeAlignment does
-  for (int i = 0; i < n; ++i) {
-    Align a;
-    alloc_align(a, ps[i].qry.size());
-    a.svType = 1234;  // "read id" hack of the caller (:363)
-    int ret = -2;
-    try {
-      ret = al->SingleAlign(i, ps[i].lines.data(), (int)ps[i].lines.size(), ps[i].ref.c_str(),
-                            ps[i].qry.c_str(), a, ps[i].qs, ps[i].qe, 0);
-    } catch (...) {
-      ret = -3;
+  // 1) one blocking SingleAlign per problem, as computeAlignment does (from `threads` worker threads)
+  {
+    const int threads = argc > 3 ? std::max(1, atoi(argv[3])) : 1;
+    std::vector<Align> as(n);
+    std::vector<int> rets(n, -2);
+    for (int i = 0; i < n; ++i) {
+      alloc_align(as[i], ps[i].qry.size());
+      as[i].svType = 1234;  // "read id" hack of the caller (:363)
     }
-    print_align("single", i, ret, a);
-    unsigned long expect = 0;
-    bool ok = true;
-    for (size_t y = 0; y < ps[i].lines.size(); ++y) {  // prepare() publishes offsetInMatrix
-      ok = ok && ps[i].lines[y].offsetInMatrix == expect;
-      expect += (unsigned long)ps[i].lines[y].length;
+    auto work = [&](int t) {
+      for (int i = t; i < n; i += threads) {
+        try {
+          rets[i] = al->SingleAlign(i, ps[i].lines.data(), (int)ps[i].lines.size(), ps[i].ref.c_str(),
+                                    ps[i].qry.c_str(), as[i], ps[i].qs, ps[i].qe, 0);
+        } catch (...) {
+          rets[i] = -3;
+        }
+      }
+    };
+    std::vector<std::thread> pool;
+    for (int t = 1; t < threads; ++t) pool.emplace_back(work, t);
+    work(0);
+    for (auto& t : pool) t.join();
+    for (int i = 0; i < n; ++i) {
+      print_align("single", i, rets[i], as[i]);
+      print_nm("single", i, rets[i], as[i]);
+      unsigned long expect = 0;
+      bool ok = true;
+      for (size_t y = 0; y < ps[i].lines.size(); ++y) {  // prepare() publishes offsetInMatrix
+        ok = ok && ps[i].lines[y].offsetInMatrix == expect;
+        expect += (unsigned long)ps[i].lines[y].length;
+      }
+      printf("offsetInMatrix %d %s\n", i, ok ? "ok" : "BAD");
+      delete[] as[i].pBuffer1; delete[] as[i].pBuffer2; delete[] as[i].nmPerPosition;
     }
-    printf("offsetInMatrix %d %s\n", i, ok ? "ok" : "BAD");
-    delete[] a.pBuffer1; delete[] a.pBuffer2; delete[] a.nmPerPosition;
   }
   // 2) the same problems through BatchAlign
   {
@@ -112,6 +148,7 @@ int main(int argc, char** argv) {
     for (int i = 0; i < n; ++i) {
       // BatchAlign reports a failed problem the way SingleAlign does: Score == -1
       print_align("batch", i, as[i].Score == -1.0f ? -1 : 0, as[i]);
+      print_nm("batch", i, as[i].Score == -1.0f ? -1 : 0, as[i]);
       delete[] as[i].pBuffer1; delete[] as[i].pBuffer2; delete[] as[i].nmPerPosition;
     }
   }
