@@ -591,6 +591,10 @@ class B200Aligner:
         """Test hook: of those, problems filled by the kernel with two rows per lane."""
         return int(self.lib.ngmlr_b200_debug_rampfree2_problems(self.h))
 
+    def debug_rampfree2_skew_problems(self):
+        """Test hook: of those, problems filled with the second row of each lane one column behind its first."""
+        return int(self.lib.ngmlr_b200_debug_rampfree2_skew_problems(self.h))
+
     def set_small_batch_teams(self, on):
         """16-warp teams for batches of at most one problem per SM (default on); see ngmlr_b200_set_small_batch_teams."""
         self.lib.ngmlr_b200_set_small_batch_teams(self.h, int(bool(on)))

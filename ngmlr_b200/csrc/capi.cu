@@ -140,6 +140,15 @@ int ngmlr_b200_create(int gpu_id, const ngmlr_b200_scoring* s, ngmlr_b200_ctx** 
       return -1;
     }
   }
+  if (const char* e = getenv("NGMLR_B200_FILL_RF2_SKEW")) {
+    if (!strcmp(e, "0")) ctx->rf2_skew = 0;
+    else if (!strcmp(e, "1")) ctx->rf2_skew = 1;
+    else {
+      g_create_error = std::string("ngmlr_b200: NGMLR_B200_FILL_RF2_SKEW=") + e + ": expected 0 or 1";
+      ngmlr_b200_destroy(ctx);
+      return -1;
+    }
+  }
   if (const char* e = getenv("NGMLR_B200_RF_TEAM_CELLS")) ctx->rf_team_cells = strtoull(e, nullptr, 10);
   if (const char* e = getenv("NGMLR_B200_FILL_CTAS_PER_SM")) ctx->fill_ctas_cap = std::max(0, atoi(e));
   if (const char* e = getenv("NGMLR_B200_NO_CORRIDOR_PACKING")) ctx->no_corridor_packing = atoi(e);
@@ -289,6 +298,9 @@ int ngmlr_b200_debug_set_big_team(ngmlr_b200_ctx* ctx, long long cells, int widt
 // two rows per lane.
 long long ngmlr_b200_debug_rampfree_problems(ngmlr_b200_ctx* ctx) { return ctx ? (long long)ctx->rf_problems : -1; }
 long long ngmlr_b200_debug_rampfree2_problems(ngmlr_b200_ctx* ctx) { return ctx ? (long long)ctx->rf2_problems : -1; }
+long long ngmlr_b200_debug_rampfree2_skew_problems(ngmlr_b200_ctx* ctx) {
+  return ctx ? (long long)ctx->rf2_skew_problems : -1;
+}
 
 // force_team: -1 auto, 0 one warp per problem, 1 four-warp teams. Test / tuning hook.
 int ngmlr_b200_set_force_team(ngmlr_b200_ctx* ctx, int v) {
@@ -355,8 +367,8 @@ int ngmlr_b200_convex_debug_directions(ngmlr_b200_ctx* ctx, int i, uint8_t* dirs
   size_t row_base = 0;
   for (size_t b = 0; b < nblk; ++b) {
     const BlockRec& br = blocks[b];
-    const int sh = f.dir_shift;
-    const size_t stride = (size_t)32 << sh, ng = (size_t)((br.nsteps + 15) / 16);
+    const int sh = f.dir_shift == 2 ? 0 : f.dir_shift;  // step offset of row t: t >> sh (device_types.h BlockRec)
+    const size_t stride = f.dir_shift ? 64 : 32, ng = (size_t)((br.nsteps + 15) / 16);
     const size_t nw = ng ? (ng - 1) * stride + 32 : 0;
     words.resize(nw);
     if (nw) CU(cudaMemcpy(words.data(), ctx->d_dir.p + br.word_off, nw * 4, cudaMemcpyDeviceToHost));

@@ -50,7 +50,7 @@ namespace nb {
 namespace {
 
 constexpr unsigned FULL = 0xffffffffu;
-constexpr int STRIP_PAD = 32;    // strip index = column + STRIP_PAD (lane 31 trails lane 0 by 31)
+constexpr int STRIP_PAD = 32;    // strip index = column + STRIP_PAD (columns >= -31 lockstep, >= -1 ramp-free)
 constexpr unsigned X_BIAS = 1u << 20;
 #ifndef FILL_TEAM_CHUNK
 #define FILL_TEAM_CHUNK 16
@@ -136,12 +136,19 @@ struct LaneState {
 // One cell (x, y) at step s. `st` is the row's state (LaneState or RowState: lL, lRunF / lIsD or lRun / lDir, kS /
 // kStep, rel); dS = S of (x-1, y-1), {nU, nP} = U and run of (x, y-1), r = the column's reference byte, q = the row's
 // read byte. Returns the direction code; {S, U, P} is what the cell below sees as its up neighbour.
-template <bool RAW, bool ALL_ACTIVE, class Row>
+// SEL_DG: pick the score, then add (both scores stay in registers) instead of a predicated second add, which the
+// compiler turns into a constant-bank load at the head of the cell's dependency chain; the same rounding either way.
+template <bool RAW, bool ALL_ACTIVE, bool SEL_DG = false, class Row>
 __device__ __forceinline__ uint32_t cell_update(Row& st, const Scoring& sc, const float dS, const float nU,
                                                 const uint32_t nP, const uint32_t r, const uint32_t q, const bool act,
                                                 const int t0rel, const int s, float& S, float& U, uint32_t& P) {
-  float dg = __fadd_rn(dS, sc.mis);
-  if (r == q) dg = __fadd_rn(dS, sc.mat);
+  float dg;
+  if (SEL_DG) {
+    dg = __fadd_rn(dS, r == q ? sc.mat : sc.mis);
+  } else {
+    dg = __fadd_rn(dS, sc.mis);
+    if (r == q) dg = __fadd_rn(dS, sc.mat);
+  }
   // Outside the corridor the cell must degenerate to {0, 0, STOP}: a NaN maximum makes every
   // equality below false, and fmaxf(NaN, 0) = 0 gives the score.
   const float m0 = fmaxf(fmaxf(fmaxf(st.lL, 0.0f), dg), nU);
@@ -669,13 +676,14 @@ __device__ __forceinline__ void rf_cols(int xlo, int xhi, unsigned rlen, int lan
   E = max(e, e1);
 }
 
-// Origin and entry step of a block from the lane's columns [A, ...). L: end of the lane's previous range (RF_NONE:
-// none); R: earliest entry; O_min: the hand-off bound.
-__device__ __forceinline__ void rf_origin(int lane, int A, int L, int R, int O_min, int& O, int& sw) {
+// Origin and entry step of a block from the lane's columns [A, ...). lag: the lane's stagger (it evaluates column x
+// at step O + lag + x); L: end of the lane's previous range (RF_NONE: none); R: earliest entry; O_min: the hand-off
+// bound.
+__device__ __forceinline__ void rf_origin(int lag, int A, int L, int R, int O_min, int& O, int& sw) {
   const int from = max(L, R);
-  const int need = A == INT_MAX ? INT_MIN : ((from + 15) & ~15) - lane - A;
+  const int need = A == INT_MAX ? INT_MIN : ((from + 15) & ~15) - lag - A;
   O = max(O_min, __reduce_max_sync(FULL, need));
-  sw = A == INT_MAX ? RF_NONE : ((O + lane + A) & ~15);
+  sw = A == INT_MAX ? RF_NONE : ((O + lag + A) & ~15);
 }
 
 // Origin and entry steps of block b (see rf_origin).
@@ -1077,7 +1085,11 @@ struct Lane2State {
   float oS, oU;  // the second row's cell: what lane t+1 (or lane 0 of the next block) reads, as in LaneState
   uint32_t oP, oC;
   float dS;      // S of (x-1, first row - 1)
-  float dS2;     // S of (x-1, first row)
+  float dS2;     // S of (x-1, first row); SKEW: of (x-2, first row)
+  // SKEW only: the first row's cell of the step before {S, U, run} (column x-1: the second row's up neighbour) and
+  // the reference byte of column x-1 (the second row's)
+  float pS, pU;
+  uint32_t pP, r1;
   RowState a, b; // first and second row
 };
 
@@ -1098,16 +1110,18 @@ __device__ __forceinline__ void row_init(RowState& r, const Scoring& sc) {
   r.rel = 0;
 }
 
-// fill_group for two rows per lane; `dwp` addresses the lane's pair of direction words of group 0.
-template <bool RAW, bool ALL_ACTIVE, int GPC, bool SELF_REF = false>
+// fill_group for two rows per lane; `dwp` addresses the lane's pair of direction words of group 0. At step s the
+// first row is at column x = s - colbase; the second row is at x too, or at x - 1 with SKEW.
+template <bool RAW, bool SKEW, bool ALL_ACTIVE, int GPC, bool SELF_REF = false>
 __device__ __forceinline__ void fill_group2(Lane2State& st, const Scoring& sc, uint4* const io_s, uint2* const dwp,
                                             const int g, const RowGeom& ga, const RowGeom& gb, const bool is31,
                                             const int src_lane, const uint8_t* ref = nullptr, int colbase = 0,
                                             unsigned ref_len = 0) {
   uint4* iop = io_s + ((g % GPC) << 5);
   uint32_t dwa = 0, dwb = 0;
+  uint32_t qa = 0, qb = 0;  // SKEW: the codes of the current 4 steps, step j at bits 2j
   {
-#pragma unroll 2
+#pragma unroll(SKEW ? 4 : 2)
     for (int k = 0; k < 16; ++k) {
       const int s = (g << 4) + k;
       uint4 v;
@@ -1119,19 +1133,50 @@ __device__ __forceinline__ void fill_group2(Lane2State& st, const Scoring& sc, u
       const bool actA = ALL_ACTIVE ? true : ((unsigned)st.a.rel < ga.rlen);
       const bool actB = ALL_ACTIVE ? true : ((unsigned)st.b.rel < gb.rlen);
       uint32_t r = v.w;
-      if (SELF_REF && !actA) r = __ldg(ref + min((unsigned)(s - colbase), ref_len));
       float SA, UA, SB, UB;
-      uint32_t PA, PB;
-      const uint32_t ca = cell_update<RAW, ALL_ACTIVE>(st.a, sc, st.dS, nU, v.z, r, ga.q, actA, ga.t0rel, s, SA, UA, PA);
-      st.dS = nS;
-      const uint32_t cb = cell_update<RAW, ALL_ACTIVE>(st.b, sc, st.dS2, UA, PA, r, gb.q, actB, gb.t0rel, s, SB, UB, PB);
-      st.dS2 = SA;
+      uint32_t PA, PB, ca, cb;
+      if (SKEW) {
+        // the two cells share no data: the second row's neighbours are all from earlier steps
+        const uint32_t rb = st.r1;
+        // outside its corridor the first row's cell does not depend on r, so the byte the lane loads there is only
+        // kept for the second row (next step): the load stays off this step's dependency chain
+        uint32_t rk = r;
+        if (SELF_REF && !actA) rk = __ldg(ref + min((unsigned)(s - colbase), ref_len));
+        ca = cell_update<RAW, ALL_ACTIVE, true>(st.a, sc, st.dS, nU, v.z, r, ga.q, actA, ga.t0rel, s, SA, UA, PA);
+        cb = cell_update<RAW, ALL_ACTIVE, true>(st.b, sc, st.dS2, st.pU, st.pP, rb, gb.q, actB, gb.t0rel, s, SB, UB,
+                                                PB);
+        st.dS = nS;
+        st.dS2 = st.pS;
+        st.pS = SA;
+        st.pU = UA;
+        st.pP = PA;
+        st.r1 = rk;
+        r = rb;  // what lane t+1 receives with the second row's cell
+      } else {
+        if (SELF_REF && !actA) r = __ldg(ref + min((unsigned)(s - colbase), ref_len));
+        ca = cell_update<RAW, ALL_ACTIVE>(st.a, sc, st.dS, nU, v.z, r, ga.q, actA, ga.t0rel, s, SA, UA, PA);
+        st.dS = nS;
+        cb = cell_update<RAW, ALL_ACTIVE>(st.b, sc, st.dS2, UA, PA, r, gb.q, actB, gb.t0rel, s, SB, UB, PB);
+        st.dS2 = SA;
+      }
       st.oS = SB;
       st.oU = UB;
       st.oP = PB;
       st.oC = r;
-      dwa = __funnelshift_r(dwa, ca, 2);
-      dwb = __funnelshift_r(dwb, cb, 2);
+      if (SKEW) {
+        // four steps' codes gathered by multiply-adds (FMA pipe), then one funnel shift per row (ALU pipe)
+        const uint32_t m = 1u << (2 * (k & 3));
+        asm("mad.lo.u32 %0, %1, %2, %3;" : "=r"(qa) : "r"(ca), "r"(m), "r"(qa));
+        asm("mad.lo.u32 %0, %1, %2, %3;" : "=r"(qb) : "r"(cb), "r"(m), "r"(qb));
+        if ((k & 3) == 3) {
+          dwa = __funnelshift_r(dwa, qa, 8);
+          dwb = __funnelshift_r(dwb, qb, 8);
+          qa = qb = 0;
+        }
+      } else {
+        dwa = __funnelshift_r(dwa, ca, 2);
+        dwb = __funnelshift_r(dwb, cb, 2);
+      }
       if (is31) {
         iop[1] = make_uint4(__float_as_uint(st.oS), __float_as_uint(st.oU), st.oP, st.oC);
         const uint4 t = iop[2];
@@ -1190,24 +1235,54 @@ __device__ __forceinline__ void rf2_cols(int xloA, int xhiA, unsigned rlenA, int
   E = max(e, e1);
 }
 
-// rf_place for 64-row block b.
-__device__ __forceinline__ void rf2_place(const CorridorView& cv, int b, int lane, int H, int ref_len, int L, int R,
-                                          int O_min, int& xloA, unsigned& rlenA, int& xloB, unsigned& rlenB, int& A,
-                                          int& E, int& O, int& sw) {
+// rf_place for 64-row block b; lag: the lane's stagger (lane, or 2 lane with SKEW).
+__device__ __forceinline__ void rf2_place(const CorridorView& cv, int b, int lane, int lag, int H, int ref_len, int L,
+                                          int R, int O_min, int& xloA, unsigned& rlenA, int& xloB, unsigned& rlenB,
+                                          int& A, int& E, int& O, int& sw) {
   int offA, lenA, offB, lenB, xhiA, xhiB;
   load_row_pair(cv, b, lane, H, offA, lenA, offB, lenB);
   row_span(offA, lenA, ref_len, xloA, xhiA, rlenA);
   row_span(offB, lenB, ref_len, xloB, xhiB, rlenB);
   rf2_cols(xloA, xhiA, rlenA, xloB, xhiB, rlenB, lane, A, E);
-  rf_origin(lane, A, L, R, O_min, O, sw);
+  rf_origin(lag, A, L, R, O_min, O, sw);
 }
 
-template <bool RAW, bool PERSIST>
+// Skewed variant (SKEW = true, the default; NGMLR_B200_FILL_RF2_SKEW=0 selects the schedule above). Lane t evaluates
+// column x of its first row at warp step O_b + 2t + x and column x - 1 of its second row in the same step, so the two
+// cell updates of a step share no data and each step's dependency chain is one cell long instead of two:
+//   first row:  up (x, 2t-1) and diagonal (x-1, 2t-1) are lane t-1's second-row cells of the step before and the one
+//               before that (the shuffle and dS, as above);
+//   second row: up (x-1, 2t) and diagonal (x-2, 2t) are the first row's cells of the step before and the one before
+//               that, left (x-2, 2t+1) is its own cell of the step before; the reference byte of x-1 is the one the
+//               first row had the step before (kept in a register, never reloaded).
+// Lane t+1's first row reaches column x one step after lane t's second row (O_b + 2t + 2 + x against O_b + 2t + 1 + x):
+// the same shuffle distances as above.
+// Both rows sweep the columns [A, E) of rf2_cols, so in first-row columns the lane runs [A, E + 1): its range ends
+// at step O_b + 2t + E + 1 (pass 1's step count and the next block's entry bound L use that end).
+// Hand-off: lane 31 trails lane 0 by 63 steps (62 of lane stagger + 1 of row skew), so its record of warp step sigma
+// is its second row's column sigma - O - 63 (the flush window). The record of column x, produced at step
+// O_{b-1} + 63 + x, is flushed at the end of its chunk; lane 0 of block b stages column x at the start of the chunk two
+// before the one holding step O_b + x. Since floor((a + 2 CHUNK) / CHUNK) = floor(a / CHUNK) + 2,
+// O_b >= O_{b-1} + 63 + 2 CHUNK is enough: RF2S_RING = 64 + 2 CHUNK.
+// Strip columns: lane 31 writes and lane 0 reads lane 31's [A, E) of rf2_cols, within [-1, refLen] as in the other
+// schedules; the stagger changes when a column passes through the strip, not which, so STRIP_PAD = 32 (>= 1) and the
+// host's STRIP_SLACK still cover it.
+// Direction words (FillOut::dir_shift = 2): the layout above (a 64-word line per group, one 8-byte store per lane) with
+// half h's BlockRec at word_off + 32 h and base = 16 * first group - O_b - 32 h, so that cell (x, 32 (2b + h) + j) lies
+// at step x - base + j (lane 16 h + (j >> 1), row j & 1: warp step O_b + 2 (16 h + (j >> 1)) + (j & 1) + x).
+// Step count: a block still advances the warp's steps by at most its column span plus the hand-off and placement
+// slack (RF2S_RING + 2 chunks + a group < 400), so the host's int guard holds unchanged.
+constexpr int RF2S_RING = 64 + 2 * RF_CHUNK;
+
+template <bool RAW, bool PERSIST, bool SKEW>
 __global__ void __launch_bounds__(FILL_WARPS_PER_CTA * 32, FILL_RF2_CTAS_PER_SM)
 convex_fill_rf2_kernel(const FillParams p) {
   constexpr int WARPS = FILL_WARPS_PER_CTA;
   constexpr int CHUNK = RF_CHUNK;
   constexpr int GPC = CHUNK / 16;
+  constexpr int RING = SKEW ? RF2S_RING : RF_RING;
+  constexpr int TAIL = SKEW ? 1 : 0;          // steps the second row runs behind the first
+  constexpr int LAG31 = SKEW ? 63 : 31;       // steps lane 31's second row trails lane 0's first row
   __shared__ uint4 s_io[WARPS][2 * (CHUNK + 1)];
   __shared__ int s_slot;
   __shared__ RfFrame s_f0[WARPS], s_f31[WARPS], s_nx[WARPS];  // as in convex_fill_rf_kernel, blk counts 64-row blocks
@@ -1229,6 +1304,7 @@ convex_fill_rf2_kernel(const FillParams p) {
   const uint4 EMPTY = make_uint4(0u, __float_as_uint(sc.open_read), empty_pack, 0u);
   const bool is0 = lane == 0, is31 = lane == 31;
   const int src_lane = (lane + 31) & 31;
+  const int lag = SKEW ? 2 * lane : lane;  // lane t's first row is at column x at step O_b + lag + x
   RfWarp& ws = s_w[wib];
 
   for (int taken = 0; PERSIST || taken < p.problems_per_cta; ++taken) {
@@ -1254,10 +1330,10 @@ convex_fill_rf2_kernel(const FillParams p) {
       for (int b = 0; b < nblk; ++b) {
         int xloA, xloB, A, E, O, sw;
         unsigned rlA, rlB;
-        rf2_place(cv, b, lane, H, (int)ref_len, L, R, O_last == RF_NONE ? INT_MIN : O_last + RF_RING, xloA, rlA, xloB,
-                  rlB, A, E, O, sw);
+        rf2_place(cv, b, lane, lag, H, (int)ref_len, L, R, O_last == RF_NONE ? INT_MIN : O_last + RING, xloA, rlA,
+                  xloB, rlB, A, E, O, sw);
         if (__any_sync(FULL, sw != RF_NONE)) O_last = O;
-        if (sw != RF_NONE) L = O + lane + E;
+        if (sw != RF_NONE) L = O + lag + E + TAIL;
         R = rf_next_entry(__reduce_max_sync(FULL, sw != RF_NONE ? sw : R - 1));
       }
       const int T = max(0, __reduce_max_sync(FULL, L));
@@ -1298,6 +1374,10 @@ convex_fill_rf2_kernel(const FillParams p) {
     st.oC = 0u;
     st.dS = 0.0f;
     st.dS2 = 0.0f;
+    st.pS = 0.0f;
+    st.pU = sc.open_read;
+    st.pP = empty_pack;
+    st.r1 = 0u;
     row_init(st.a, sc);
     row_init(st.b, sc);
     RowGeom ga, gb;  // before its first rows a lane is outside every corridor
@@ -1313,8 +1393,8 @@ convex_fill_rf2_kernel(const FillParams p) {
       const int ks = second ? st.b.kStep : st.a.kStep;
       const float kS = second ? st.b.kS : st.a.kS;
       if (ks >= 0)
-        s_bestl[wib][lane] = make_float4(kS, __int_as_float(ks - me.x - lane), __int_as_float(me.y + (second ? 1 : 0)),
-                                         0.0f);
+        s_bestl[wib][lane] = make_float4(kS, __int_as_float(ks - me.x - lag - (second ? TAIL : 0)),
+                                         __int_as_float(me.y + (second ? 1 : 0)), 0.0f);
       st.a.kS = st.b.kS = kS;
       st.a.kStep = st.b.kStep = -1;
     };
@@ -1327,15 +1407,16 @@ convex_fill_rf2_kernel(const FillParams p) {
       int4 me = s_cur[wib][lane];
       int xloA, xloB, A, E, O, swl;
       unsigned rlA, rlB;
-      rf2_place(cv, b, lane, H, (int)ref_len, me.z, R, O_last == RF_NONE ? INT_MIN : O_last + RF_RING, xloA, rlA, xloB,
-                rlB, A, E, O, swl);
+      rf2_place(cv, b, lane, lag, H, (int)ref_len, me.z, R, O_last == RF_NONE ? INT_MIN : O_last + RING, xloA, rlA,
+                xloB, rlB, A, E, O, swl);
       const bool any = __any_sync(FULL, swl != RF_NONE);
-      if (swl != RF_NONE) me.z = O + lane + E;
+      if (swl != RF_NONE) me.z = O + lag + E + TAIL;
       me.w += (int)(rlA + rlB);
       const int swmax = __reduce_max_sync(FULL, swl != RF_NONE ? swl : R - 1);
       const int y = (b << 6) + 2 * lane;
-      const int4 na = make_int4(swl - (O + lane + xloA), (int)rlA, y < H ? (int)p.seq[dp->qry_off + y] : 0x100, 0);
-      const int4 nb2 = make_int4(swl - (O + lane + xloB), (int)rlB, y + 1 < H ? (int)p.seq[dp->qry_off + y + 1] : 0x100, 0);
+      const int4 na = make_int4(swl - (O + lag + xloA), (int)rlA, y < H ? (int)p.seq[dp->qry_off + y] : 0x100, 0);
+      const int4 nb2 = make_int4(swl - (O + lag + xloB) - TAIL, (int)rlB,
+                                 y + 1 < H ? (int)p.seq[dp->qry_off + y + 1] : 0x100, 0);
       // the first row of the block with a cell (rows 2t, 2t + 1 of lane t in row-major order)
       const int key = rlA ? 2 * lane : (rlB ? 2 * lane + 1 : INT_MAX);
       const int kmin = __reduce_min_sync(FULL, key);
@@ -1357,7 +1438,7 @@ convex_fill_rf2_kernel(const FillParams p) {
         }
       }
       const int g0 = __reduce_min_sync(FULL, swl != RF_NONE ? swl : INT_MAX);
-      const int end = __reduce_max_sync(FULL, swl != RF_NONE ? O + lane + E : INT_MIN);
+      const int end = __reduce_max_sync(FULL, swl != RF_NONE ? O + lag + E + TAIL : INT_MIN);
       const int a31 = __shfl_sync(FULL, A, 31), e31 = __shfl_sync(FULL, E, 31);
       const int sw0 = __shfl_sync(FULL, swl, 0), sw31 = __shfl_sync(FULL, swl, 31);
       s_cur[wib][lane] = me;
@@ -1370,7 +1451,7 @@ convex_fill_rf2_kernel(const FillParams p) {
         for (int h = 0; h < 2 && 2 * b + h < nblk32; ++h) {
           BlockRec br;
           br.word_off = ws.word_off + (any ? (unsigned long long)(g0 >> 4) * 64ull : 0ull) + 32ull * h;
-          br.base = any ? g0 - O - 16 * h : 0;
+          br.base = any ? g0 - O - (SKEW ? 32 : 16) * h : 0;
           br.nsteps = any ? end - g0 : 0;
           p.blocks[dp->blk_off + 2 * b + h] = br;
         }
@@ -1469,10 +1550,10 @@ convex_fill_rf2_kernel(const FillParams p) {
         const bool all_active = __all_sync(FULL, st.a.rel >= 0 && st.a.rel + 15 < (int)ga.rlen && st.b.rel >= 0 &&
                                                      st.b.rel + 15 < (int)gb.rlen);
         if (all_active) {
-          fill_group2<RAW, true, GPC>(st, sc, io_s, dwp, g, ga, gb, is31, src_lane);
+          fill_group2<RAW, SKEW, true, GPC>(st, sc, io_s, dwp, g, ga, gb, is31, src_lane);
         } else {
-          fill_group2<RAW, false, GPC, true>(st, sc, io_s, dwp, g, ga, gb, is31, src_lane, ref,
-                                              s_cur[wib][lane].x + lane, ref_len);
+          fill_group2<RAW, SKEW, false, GPC, true>(st, sc, io_s, dwp, g, ga, gb, is31, src_lane, ref,
+                                                    s_cur[wib][lane].x + lag, ref_len);
         }
       }
       __syncwarp();
@@ -1487,7 +1568,7 @@ convex_fill_rf2_kernel(const FillParams p) {
           const int sigma = c * CHUNK + j;
           const bool in_n = n->blk >= 0 && n->sw31 != RF_NONE && sigma >= n->sw31;
           const RfFrame* fr = in_n ? n : f;
-          const int x = sigma - fr->O - 31;
+          const int x = sigma - fr->O - LAG31;
           if (j < done && (in_n || f->blk >= 0) && x >= fr->a31 && x < fr->e31) st_strip(strip + x, io_s[2 * j + 1]);
         }
       }
@@ -1537,7 +1618,7 @@ convex_fill_rf2_kernel(const FillParams p) {
       o.best_y = bestY;
       o.status = status;
       o.cells = cells;
-      o.dir_shift = 1;
+      o.dir_shift = SKEW ? 2 : 1;
       p.out[ai] = o;
     }
     __syncwarp();
@@ -1558,11 +1639,11 @@ void launch_fill_rf(const FillParams& p, int grid, cudaStream_t stream) {
   else convex_fill_rf_kernel<RAW, true><<<grid, threads, 0, stream>>>(p);
 }
 
-template <bool RAW>
+template <bool RAW, bool SKEW>
 void launch_fill_rf2(const FillParams& p, int grid, cudaStream_t stream) {
   const int threads = FILL_WARPS_PER_CTA * 32;
-  if (p.sm_slots) convex_fill_rf2_kernel<RAW, false><<<grid, threads, 0, stream>>>(p);
-  else convex_fill_rf2_kernel<RAW, true><<<grid, threads, 0, stream>>>(p);
+  if (p.sm_slots) convex_fill_rf2_kernel<RAW, false, SKEW><<<grid, threads, 0, stream>>>(p);
+  else convex_fill_rf2_kernel<RAW, true, SKEW><<<grid, threads, 0, stream>>>(p);
 }
 
 template <bool RAW, int NW>
@@ -1575,9 +1656,12 @@ void launch_fill(const FillParams& p, int grid, cudaStream_t stream) {
 
 // p.sm_slots != nullptr selects the short-lived-CTA instantiation (one problem per warp / team, strips by SM slot)
 cudaError_t launch_convex_fill(const FillParams& p, bool raw, bool team, int rampfree, int grid, cudaStream_t stream) {
-  if (rampfree == 2) {
-    if (raw) launch_fill_rf2<true>(p, grid, stream);
-    else launch_fill_rf2<false>(p, grid, stream);
+  if (rampfree == 3) {
+    if (raw) launch_fill_rf2<true, true>(p, grid, stream);
+    else launch_fill_rf2<false, true>(p, grid, stream);
+  } else if (rampfree == 2) {
+    if (raw) launch_fill_rf2<true, false>(p, grid, stream);
+    else launch_fill_rf2<false, false>(p, grid, stream);
   } else if (rampfree) {
     if (raw) launch_fill_rf<true>(p, grid, stream);
     else launch_fill_rf<false>(p, grid, stream);
@@ -1602,8 +1686,10 @@ int fill_max_ctas_per_sm(bool raw, bool team, int rampfree) {
   int n = 0;
   const int threads = FILL_WARPS_PER_CTA * 32;
   auto occ = [&](auto kernel) { cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, kernel, threads, 0); };
-  if (rampfree == 2) {
-    raw ? occ(convex_fill_rf2_kernel<true, true>) : occ(convex_fill_rf2_kernel<false, true>);
+  if (rampfree == 3) {
+    raw ? occ(convex_fill_rf2_kernel<true, true, true>) : occ(convex_fill_rf2_kernel<false, true, true>);
+  } else if (rampfree == 2) {
+    raw ? occ(convex_fill_rf2_kernel<true, true, false>) : occ(convex_fill_rf2_kernel<false, true, false>);
   } else if (rampfree) {
     raw ? occ(convex_fill_rf_kernel<true, true>) : occ(convex_fill_rf_kernel<false, true>);
   } else if (raw) {

@@ -178,7 +178,9 @@ int convex_upload_spec(ngmlr_b200_ctx* ctx, const UploadSpec& sp) {
       const long long steps = w + 31 + adv, steps_rf = std::max<long long>(steps, RF_MIN_BLOCK_STEPS);
       dirw[i] = (size_t)(((size_t)ql + 31) / 32) * (size_t)((steps + 15) / 16 + 1) * 32;
       if (ctx->rows_per_lane == 2) {  // 64-row blocks, 64 words per group; the hand-off spacing is per block as well
-        const long long steps2 = std::max<long long>(w + 31 + 2 * adv, RF_MIN_BLOCK_STEPS);
+        // skewed: lane 31's second row trails lane 0 by 63 steps, and the hand-off spacing is 32 steps longer
+        const long long steps2 = ctx->rf2_skew ? std::max<long long>(w + 63 + 2 * adv, RF2S_MIN_BLOCK_STEPS)
+                                               : std::max<long long>(w + 31 + 2 * adv, RF_MIN_BLOCK_STEPS);
         dirw_rf[i] = (size_t)(((size_t)ql + 63) / 64) * (size_t)((steps2 + 15) / 16 + 1) * 64;
       } else {
         dirw_rf[i] = (size_t)(((size_t)ql + 31) / 32) * (size_t)((steps_rf + 15) / 16 + 1) * 32;
@@ -441,10 +443,11 @@ int ngmlr_b200_convex_run(ngmlr_b200_ctx* ctx) {
   // problems still get 4-warp teams, in a launch of their own (below). NGMLR_B200_FILL_TEAM=1 selects the ramped
   // teams for everything, NGMLR_B200_FILL_SCHEDULE=ramped the ramped kernels everywhere (DESIGN.md section 4.1).
   // (fill_schedule 2, NGMLR_B200_FILL_SCHEDULE=rampfree-all: every batch, whatever its widths -- test / tuning hook)
-  // NGMLR_B200_FILL_ROWS_PER_LANE picks its kernel: 64-row blocks with two rows per lane (default) or 32-row blocks.
+  // NGMLR_B200_FILL_ROWS_PER_LANE picks its kernel: 64-row blocks with two rows per lane (default) or 32-row blocks;
+  // NGMLR_B200_FILL_RF2_SKEW=0 runs the two rows of a lane in the same column instead of the second one behind.
   const bool rf_on = ctx->fill_schedule >= 1 && ctx->force_team != 1 && ctx->rf_fits &&
                      (ctx->fill_schedule == 2 || ctx->rf_wide * 2 > n);
-  const int rampfree = rf_on ? ctx->rows_per_lane : 0;
+  const int rampfree = !rf_on ? 0 : ctx->rows_per_lane == 1 ? 1 : ctx->rf2_skew ? 3 : 2;
   if (rampfree) team = false;
   const int variant = (raw ? 1 : 0) | (team ? 2 : 0) | (rampfree << 2);
   if (!ctx->ctas_per_sm[variant]) ctx->ctas_per_sm[variant] = std::max(1, fill_max_ctas_per_sm(raw, team, rampfree));
@@ -664,7 +667,8 @@ int ngmlr_b200_convex_run(ngmlr_b200_ctx* ctx) {
   }
   words_needed = std::max(words_needed, (size_t)ctx->dir_used);
   if (rampfree) ctx->rf_problems += (unsigned long long)(n - n_big - n_team);
-  if (rampfree == 2) ctx->rf2_problems += (unsigned long long)(n - n_big - n_team);
+  if (rampfree >= 2) ctx->rf2_problems += (unsigned long long)(n - n_big - n_team);
+  if (rampfree == 3) ctx->rf2_skew_problems += (unsigned long long)(n - n_big - n_team);
   float ms = 0;
   cudaEventElapsedTime(&ms, ctx->ev[0], ctx->ev[1]);
   ctx->stats.fill_ms = ms;

@@ -38,8 +38,8 @@ struct RowWindow {
 // walk's loop.
 template <int SH>
 __device__ __forceinline__ void trace_problem(const TraceParams& p, const int i, const int lane) {
-  constexpr int sh = SH;
-  constexpr unsigned stride = 32u << SH;
+  constexpr int sh = SH == 2 ? 0 : SH;  // step offset of row t of a block: t >> sh
+  constexpr unsigned stride = SH ? 64u : 32u;
   const AlnDesc d = p.desc[i];
   const FillOut f = p.fill[i];
   TraceOut o;
@@ -293,7 +293,9 @@ __global__ void __launch_bounds__(TB_WARPS_PER_CTA * 32) convex_traceback_kernel
   const int lane = threadIdx.x & 31;
   if (slot >= p.n) return;
   const int i = p.order[slot];  // longest walks first: no straggler warps at the end of the launch
-  if (p.fill[i].dir_shift) trace_problem<1>(p, i, lane);
+  const int sh = p.fill[i].dir_shift;
+  if (sh == 2) trace_problem<2>(p, i, lane);
+  else if (sh) trace_problem<1>(p, i, lane);
   else trace_problem<0>(p, i, lane);
 }
 

@@ -55,6 +55,7 @@ struct alignas(16) AlnDesc {
 //   dir[word_off + (s >> 4) * (32 << k) + t] >> ((s & 15) * 2),
 // k = FillOut::dir_shift: 0 for the kernels with one row per lane, 1 for the one with two (a lane's two rows share a
 // step; its 16-step group of a 64-row block is one 64-word line, and the second 32-row half starts at word 32).
+// k = 2, the two-row kernel with the second row one column behind: 64-word lines as for 1, s = x - base + t.
 struct alignas(16) BlockRec {
   uint64_t word_off;
   int32_t base;

@@ -25,13 +25,15 @@ constexpr int FILL_BIG_TEAM = 16;  // warps that pipeline one huge matrix (one C
 
 constexpr int RF_MIN_WIDTH = 128;  // one-warp launches take the ramp-free schedule when most corridors are this wide
 constexpr int RF_MIN_BLOCK_STEPS = 224;  // steps per 32-row block the ramp-free schedule may spend on a narrow corridor
+// the same per 64-row block of the skewed two-row kernel: its hand-off spacing is 32 steps longer
+constexpr int RF2S_MIN_BLOCK_STEPS = RF_MIN_BLOCK_STEPS + 32;
 // with the ramp-free schedule, problems of at least this many cells are filled by FILL_WARPS_PER_CTA-warp teams in a
 // launch of their own: one warp would still be busy with them long after the rest of the batch is done
 constexpr unsigned long long RF_TEAM_CELLS = 8ull << 20;
 
 // team = all FILL_WARPS_PER_CTA warps of a CTA pipeline one problem; otherwise one warp per problem.
-// rampfree 1 / 2: one warp per problem in the ramp-free row schedule with one / two rows per lane (convex_fill.cu;
-// `team` is ignored); 0: the ramped kernels.
+// rampfree 1 / 2 / 3: one warp per problem in the ramp-free row schedule with one / two rows per lane / two rows per
+// lane, the second one column behind the first (convex_fill.cu; `team` is ignored); 0: the ramped kernels.
 cudaError_t launch_convex_fill(const FillParams& p, bool raw, bool team, int rampfree, int grid, cudaStream_t stream);
 // the same kernel with a FILL_BIG_TEAM-warp team per problem, for the huge matrices of a batch
 cudaError_t launch_convex_fill_big(const FillParams& p, bool raw, int grid, cudaStream_t stream);

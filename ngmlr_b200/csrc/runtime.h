@@ -222,7 +222,9 @@ struct ngmlr_b200_ctx {
   bool rf_fits = true;    // every problem's ramp-free step count fits the kernel's int step numbers
   unsigned long long rf_problems = 0;  // problems filled by the ramp-free kernels since the context was created
   unsigned long long rf2_problems = 0; // of those, by the kernel with two rows per lane
+  unsigned long long rf2_skew_problems = 0;  // of those, in its skewed schedule
   int rows_per_lane = 2;  // rows per lane of the ramp-free kernel: 1 or 2 (NGMLR_B200_FILL_ROWS_PER_LANE)
+  int rf2_skew = 1;       // two rows per lane: the second row one column behind the first (NGMLR_B200_FILL_RF2_SKEW)
   int rf_team = 0;        // problems after the big ones with >= rf_team_cells cells (they lead the order)
   unsigned long long rf_team_cells = nb::RF_TEAM_CELLS;  // NGMLR_B200_RF_TEAM_CELLS
   int fill_schedule = 1;  // 1: ramp-free row schedule where it applies, 2: for every batch, 0: ramped (NGMLR_B200_FILL_SCHEDULE)
@@ -230,7 +232,7 @@ struct ngmlr_b200_ctx {
   nb::PinBuf<unsigned long long> h_win;   // decode_windows: start | arena offset | (sequenceLength, span) pairs
   nb::DevBuf<unsigned long long> d_win;
   int64_t upload_d2h_bytes = 0;
-  int ctas_per_sm[12] = {};  // occupancy of the fill-kernel variants (raw x team x ramped / ramp-free 1 or 2 rows)
+  int ctas_per_sm[16] = {};  // occupancy of the fill-kernel variants (raw x team x launch_convex_fill's rampfree)
   long long debug_arena_words = -1;    // test hook: initial direction-arena size
   // Test hook (ngmlr_b200_debug_set_arena_cap, NGMLR_B200_DEBUG_ARENA_CAP): the device arenas of convex batches may
   // hold at most this many bytes (-1: no cap). A reservation beyond it fails the way cudaMalloc does when the device

@@ -3,16 +3,17 @@
 --cpu (the default) counts, from the bench workload's own corridors, the lane-steps each schedule issues per DP
 cell: the ramped kernel's block_geom arithmetic, and the ramp-free kernels' placement rule restated here (entry at
 a 16-step group boundary, no overlap within a lane, one chunk between a block's last entry and the next block's
-first, the hand-off spacing O_b >= O_{b-1} + RF_RING), for 32-row blocks and for 64-row blocks with two rows per lane.
-A lane-step of the two-row kernel evaluates two cells; "rampfree2" counts cell slots (2 per lane-step) per cell, so the
-three figures compare idle work. No GPU is needed.
+first, the hand-off spacing O_b >= O_{b-1} + RF_RING), for 32-row blocks and for 64-row blocks with two rows per lane,
+the latter with both rows in the same column and with the second one column behind (lane stagger 2, RF2S_RING).
+A lane-step of the two-row kernels evaluates two cells; "rampfree2" and "rampfree2-skew" count cell slots (2 per
+lane-step) per cell, so the figures compare idle work. No GPU is needed.
 
---gpu runs `bench.py --profile-only` and the full `bench.py` under NGMLR_B200_FILL_SCHEDULE=ramped, and =rampfree
-with NGMLR_B200_FILL_ROWS_PER_LANE=1 and =2, alternating, and prints the medians and spreads of the fill kernel time
-and of the headline value, with the card name, power limit and SM clock read in the same run.
+--gpu runs `bench.py --profile-only` and the full `bench.py` under each of --settings (default: all of them),
+alternating, and prints the medians and spreads of the fill kernel time and of the headline value, with the card name,
+power limit and SM clock read in the same run. --dump-outputs also writes each setting's bench outputs once.
 
     python scripts/fill_schedule.py --cpu [--reads 300]
-    python scripts/fill_schedule.py --gpu --runs 3 --out DIR
+    python scripts/fill_schedule.py --gpu --runs 3 --out DIR [--settings rampfree-rows2,rampfree-rows2-skew]
 """
 import argparse
 import json
@@ -28,6 +29,7 @@ sys.path.insert(0, ROOT)
 INT_MAX = 2**31 - 1
 RF_CHUNK = 64                  # steps staged per chunk (RF_CHUNK)
 RF_RING = 32 + 2 * RF_CHUNK    # hand-off spacing of consecutive origins (RF_RING)
+RF2S_RING = 64 + 2 * RF_CHUNK  # the same for the skewed two-row schedule (RF2S_RING)
 
 
 def spans(offs, lens, ref_len, b, H):
@@ -82,10 +84,13 @@ def rf2_cols(offs, lens, ref_len, b, H):
     return A, E
 
 
-def rampfree_steps(offs, lens, ref_len, rows=1):
-    """Steps of the warp under the ramp-free placement (pass 1 of convex_fill_rf_kernel / convex_fill_rf2_kernel)."""
+def rampfree_steps(offs, lens, ref_len, rows=1, skew=False):
+    """Steps of the warp under the ramp-free placement (pass 1 of convex_fill_rf_kernel / convex_fill_rf2_kernel).
+    skew: lane t's first row is at column x at step O + 2t + x and its second row one column behind, so its range
+    ends one step later."""
     H = len(offs)
-    lane = np.arange(32)
+    lane = np.arange(32) * (2 if skew else 1)
+    tail, ring = (1, RF2S_RING) if skew else (0, RF_RING)
     L = np.full(32, -INT_MAX, dtype=np.int64)
     R, O_last = 0, None
     per = 32 * rows
@@ -99,12 +104,12 @@ def rampfree_steps(offs, lens, ref_len, rows=1):
         need = np.where(has, ((frm + 15) // 16) * 16 - lane - A, -INT_MAX)
         O = int(need.max())
         if O_last is not None:
-            O = max(O, O_last + RF_RING)
+            O = max(O, O_last + ring)
         sw = np.where(has, ((O + lane + A) // 16) * 16, -INT_MAX)
         assert (sw[has] >= L[has]).all() and (sw[has] <= (O + lane + A)[has]).all()
         if has.any():
             O_last = O
-        L = np.where(has, O + lane + E, L)
+        L = np.where(has, O + lane + E + tail, L)
         swmax = int(sw[has].max()) if has.any() else R - 1
         R = ((swmax + RF_CHUNK) // RF_CHUNK + 1) * RF_CHUNK
     return (max(0, int(L.max())) + 15) // 16 * 16
@@ -116,7 +121,7 @@ def cpu(args):
     contig = 10_000_000
     genome = synth.random_genome(5 * contig, 1)
     reads, ivs = synth.simulate_reads(args.reads, genome, contig, 3, **cfg)
-    cells = ramp = rf = rf2 = 0
+    cells = ramp = rf = rf2 = rf2s = 0
     widths = []
     for iv in ivs:
         p = iv.problem(genome, reads)
@@ -128,6 +133,7 @@ def cpu(args):
         ramp += 32 * ramped_steps(offs, lens, ref_len)
         rf += 32 * rampfree_steps(offs, lens, ref_len)
         rf2 += 64 * rampfree_steps(offs, lens, ref_len, rows=2)
+        rf2s += 64 * rampfree_steps(offs, lens, ref_len, rows=2, skew=True)
     w = np.array(widths)
     out = {
         "problems": len(ivs),
@@ -136,6 +142,7 @@ def cpu(args):
             "ramped": round(ramp / cells, 4),
             "rampfree": round(rf / cells, 4),
             "rampfree2": round(rf2 / cells, 4),
+            "rampfree2-skew": round(rf2s / cells, 4),
         },
     }
     print(json.dumps(out, indent=1))
@@ -147,14 +154,17 @@ def smi():
     return r.stdout.strip().splitlines()[0] if r.returncode == 0 and r.stdout.strip() else "nvidia-smi unavailable"
 
 
-SETTINGS = {"ramped": ("ramped", "1"), "rampfree-rows1": ("rampfree", "1"), "rampfree-rows2": ("rampfree", "2")}
+# schedule, rows per lane, skew of the two-row kernel
+SETTINGS = {"ramped": ("ramped", "1", "0"), "rampfree-rows1": ("rampfree", "1", "0"),
+            "rampfree-rows2": ("rampfree", "2", "0"), "rampfree-rows2-skew": ("rampfree", "2", "1")}
 
 
-def bench(setting, extra, steps, warmup):
-    schedule, rows = SETTINGS[setting]
-    env = dict(os.environ, NGMLR_B200_FILL_SCHEDULE=schedule, NGMLR_B200_FILL_ROWS_PER_LANE=rows)
+def bench(setting, extra, steps, warmup, config):
+    schedule, rows, skew = SETTINGS[setting]
+    env = dict(os.environ, NGMLR_B200_FILL_SCHEDULE=schedule, NGMLR_B200_FILL_ROWS_PER_LANE=rows,
+               NGMLR_B200_FILL_RF2_SKEW=skew)
     cmd = [sys.executable, os.path.join(ROOT, "bench.py"), "--gpus", "1", "--steps", str(steps),
-           "--warmup", str(warmup)] + extra
+           "--warmup", str(warmup), "--config", config] + extra
     r = subprocess.run(cmd, env=env, capture_output=True, text=True, cwd=ROOT)
     lines = [l for l in r.stdout.splitlines() if l.startswith("{")]
     if r.returncode != 0 or not lines:
@@ -164,25 +174,30 @@ def bench(setting, extra, steps, warmup):
 
 def gpu(args):
     print("card:", smi())
-    res = {k: {"prof": [], "full": []} for k in SETTINGS}
+    settings = args.settings.split(",") if args.settings else list(SETTINGS)
+    res = {k: {"prof": [], "full": []} for k in settings}
     for i in range(args.runs):
-        for sched in SETTINGS:
-            prof = bench(sched, ["--profile-only"], args.steps, args.warmup)
-            full = bench(sched, [], args.steps, args.warmup)
+        for sched in settings:
+            dump = ["--dump-outputs", os.path.join(args.out, "dump", sched)] if args.dump_outputs and i == 0 else []
+            prof = bench(sched, ["--profile-only"], args.steps, args.warmup, args.config) if not args.full_only else None
+            full = bench(sched, dump, args.steps, args.warmup, args.config)
             res[sched]["prof"].append(prof)
             res[sched]["full"].append(full)
             print(f"run {i} {sched}: fill {full['kernel_ms_per_step']['fill']:.2f} ms/step, value {full['value']:.4f}, "
                   f"parity {full.get('parity_checked')}", flush=True)
-    summary = {"card": smi()}
+    summary = {"card": smi(), "config": args.config}
     for sched, r in res.items():
         fill = np.array([x["kernel_ms_per_step"]["fill"] for x in r["full"]])
         val = np.array([x["value"] for x in r["full"]])
-        pfill = np.array([x["fill_ms"] for x in r["prof"]])
         summary[sched] = {"fill_ms_median": float(np.median(fill)), "fill_ms_spread": float(fill.max() - fill.min()),
                           "value_median": float(np.median(val)), "value_spread": float(val.max() - val.min()),
-                          "solo_fill_ms_median": float(np.median(pfill)), "fill_ms": fill.tolist(),
-                          "value": val.tolist()}
-    for a, b in (("ramped", "rampfree-rows1"), ("rampfree-rows1", "rampfree-rows2")):
+                          "fill_ms": fill.tolist(), "value": val.tolist()}
+        if not args.full_only:
+            pfill = np.array([x["fill_ms"] for x in r["prof"]])
+            summary[sched].update(solo_fill_ms_median=float(np.median(pfill)),
+                                  solo_fill_ms_spread=float(pfill.max() - pfill.min()), solo_fill_ms=pfill.tolist())
+    pairs = (("ramped", "rampfree-rows1"), ("rampfree-rows1", "rampfree-rows2"), ("rampfree-rows2", "rampfree-rows2-skew"))
+    for a, b in (ab for ab in pairs if ab[0] in res and ab[1] in res):
         summary[f"fill_change {a} -> {b}"] = summary[b]["fill_ms_median"] / summary[a]["fill_ms_median"] - 1.0
         summary[f"value_change {a} -> {b}"] = summary[b]["value_median"] / summary[a]["value_median"] - 1.0
     print(json.dumps(summary, indent=1))
@@ -201,7 +216,13 @@ def main():
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=2)
     ap.add_argument("--out", default=None)
+    ap.add_argument("--settings", default=None, help="comma-separated subset of " + ", ".join(SETTINGS))
+    ap.add_argument("--config", default="pacbio50", help="bench.py --config")
+    ap.add_argument("--full-only", action="store_true", help="skip the --profile-only runs")
+    ap.add_argument("--dump-outputs", action="store_true", help="bench.py --dump-outputs OUT/dump/SETTING, first run")
     args = ap.parse_args()
+    if args.dump_outputs and not args.out:
+        ap.error("--dump-outputs needs --out")
     if args.gpu:
         gpu(args)
     if args.cpu or not args.gpu:
