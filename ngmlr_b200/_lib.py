@@ -116,6 +116,7 @@ def load():
     lib.ngmlr_b200_debug_rampfree2_problems.restype = C.c_longlong
     lib.ngmlr_b200_debug_rampfree2_skew_problems.argtypes = [vp]
     lib.ngmlr_b200_debug_rampfree2_skew_problems.restype = C.c_longlong
+    lib.ngmlr_b200_debug_fill_counts.argtypes = [vp, C.POINTER(C.c_longlong), C.c_int]
     lib.ngmlr_b200_debug_set_big_team.argtypes = [vp, C.c_longlong, C.c_int]
     batch = [vp, C.c_int, cpp, i32p, cpp, i32p, i32p, i32p, i64p, i32p, i32p]
     lib.ngmlr_b200_convex_upload.argtypes = batch

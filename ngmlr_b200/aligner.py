@@ -595,6 +595,19 @@ class B200Aligner:
         """Test hook: of those, problems filled with the second row of each lane one column behind its first."""
         return int(self.lib.ngmlr_b200_debug_rampfree2_skew_problems(self.h))
 
+    FILL_COUNTS = ("big_team", "rf_team", "rampfree", "ramped_warp", "ramped_team", "raw",
+                   "fill_launches", "multi_launch", "three_way")
+
+    def debug_fill_counts(self):
+        """Test hook: the fill's routing counters since the aligner was created -- problems filled by the 16-warp launch
+        (big_team), the ramp-free schedule's concurrent 4-warp team launch (rf_team), the ramp-free kernels (rampfree),
+        the ramped one-warp and 4-warp team kernels of the ordinary launch (ramped_warp, ramped_team) and the RAW
+        instantiation in any launch (raw); fill launches, those with more than one of the three concurrent launches
+        non-empty (multi_launch) and those with all three (three_way)."""
+        out = (C.c_longlong * len(self.FILL_COUNTS))()
+        self._check(self.lib.ngmlr_b200_debug_fill_counts(self.h, out, len(out)))
+        return dict(zip(self.FILL_COUNTS, (int(v) for v in out)))
+
     def set_small_batch_teams(self, on):
         """16-warp teams for batches of at most one problem per SM (default on); see ngmlr_b200_set_small_batch_teams."""
         self.lib.ngmlr_b200_set_small_batch_teams(self.h, int(bool(on)))

@@ -302,6 +302,20 @@ long long ngmlr_b200_debug_rampfree2_skew_problems(ngmlr_b200_ctx* ctx) {
   return ctx ? (long long)ctx->rf2_skew_problems : -1;
 }
 
+// Test hook: the fill's routing counters since the context was created, out[0..min(n, 9)) = problems filled by the
+// 16-warp launch, by the ramp-free schedule's 4-warp team launch, by the ramp-free kernels, by the ramped one-warp
+// kernel, by the ramped 4-warp team kernel (ordinary launch), by the RAW instantiation; fill launches, those with more
+// than one of the three concurrent launches non-empty, and those with all three. Returns the number of entries written.
+int ngmlr_b200_debug_fill_counts(ngmlr_b200_ctx* ctx, long long* out, int n) {
+  if (!ctx || !out) return -1;
+  const unsigned long long v[9] = {ctx->big_team_problems,    ctx->rf_team_problems,    ctx->rf_problems,
+                                   ctx->ramped_warp_problems, ctx->ramped_team_problems, ctx->raw_problems,
+                                   ctx->fill_launch_count,    ctx->multi_launch_count,  ctx->three_way_launch_count};
+  const int k = std::max(0, std::min(n, 9));
+  for (int i = 0; i < k; ++i) out[i] = (long long)v[i];
+  return k;
+}
+
 // force_team: -1 auto, 0 one warp per problem, 1 four-warp teams. Test / tuning hook.
 int ngmlr_b200_set_force_team(ngmlr_b200_ctx* ctx, int v) {
   if (!ctx) return -1;

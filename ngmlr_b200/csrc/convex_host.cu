@@ -219,6 +219,14 @@ int convex_upload_spec(ngmlr_b200_ctx* ctx, const UploadSpec& sp) {
     big[i] = est[i] >= ctx->big_cells && maxlen[i] >= ctx->big_width;
     n_big += big[i];
   }
+  // No FILL_BIG_TEAM-warp launch when teams are off, or for a batch mostly of huge problems (4-warp teams fill the
+  // GPU better): then no problem leads the order as big, and the team count below covers every problem of at least
+  // rf_team_cells cells -- the ramp-free schedule's team launch takes them all, as it does beside a big-team launch.
+  const bool big_ok = ctx->team_safe && ctx->force_team != 0 && !getenv("NGMLR_B200_NO_BIG_TEAMS");
+  if (!big_ok || (n_big > 2 * ctx->num_sms && n_big * 2 > n)) {
+    std::fill(big.begin(), big.end(), (uint8_t)0);
+    n_big = 0;
+  }
   ctx->n_big = n_big;
   ctx->rf_team = 0;
   for (int i = 0; i < n; ++i) ctx->rf_team += !big[i] && est[i] >= ctx->rf_team_cells;
@@ -473,10 +481,10 @@ int ngmlr_b200_convex_run(ngmlr_b200_ctx* ctx) {
     }
   }
   const size_t bnd_stride = align_up((size_t)ctx->max_ref_len + STRIP_SLACK, 8);
-  // huge matrices: their own launch with FILL_BIG_TEAM-warp teams, concurrent with the rest (second stream)
+  // huge matrices: their own launch with FILL_BIG_TEAM-warp teams, concurrent with the rest (second stream); whether
+  // the batch has one is decided at upload, where the order is built
   const bool big_ok = ctx->team_safe && ctx->force_team != 0 && !getenv("NGMLR_B200_NO_BIG_TEAMS");
   int n_big = big_ok ? ctx->n_big : 0;
-  if (n_big > 2 * ctx->num_sms && n_big * 2 > n) n_big = 0;  // a batch of huge problems only: 4-warp teams fill the GPU
   // A batch smaller than the GPU (the plugin's SingleAlign batches: a handful of blocking callers) is latency, not
   // throughput: every problem gets an SM and a 16-warp team of its own.
   if (big_ok && n <= ctx->num_sms && ctx->small_batch_big_teams) n_big = n;
@@ -596,6 +604,10 @@ int ngmlr_b200_convex_run(ngmlr_b200_ctx* ctx) {
       CU(cudaEventRecord(ctx->ev[2], st));
       ctx->stats.fill_launches++;
       ctx->stats.traceback_launches++;
+      const int launches = (n_big > 0) + (n_team > 0) + (n_rest > 0);
+      ctx->fill_launch_count++;
+      ctx->multi_launch_count += launches > 1;
+      ctx->three_way_launch_count += launches == 3;
     }
     if (dev_text) {
       CU(ctx->arena_reserve(ctx->d_text, text_cap));
@@ -669,6 +681,10 @@ int ngmlr_b200_convex_run(ngmlr_b200_ctx* ctx) {
   if (rampfree) ctx->rf_problems += (unsigned long long)(n - n_big - n_team);
   if (rampfree >= 2) ctx->rf2_problems += (unsigned long long)(n - n_big - n_team);
   if (rampfree == 3) ctx->rf2_skew_problems += (unsigned long long)(n - n_big - n_team);
+  ctx->big_team_problems += (unsigned long long)n_big;
+  ctx->rf_team_problems += (unsigned long long)n_team;
+  if (!rampfree) (team ? ctx->ramped_team_problems : ctx->ramped_warp_problems) += (unsigned long long)(n - n_big - n_team);
+  if (raw) ctx->raw_problems += (unsigned long long)n;
   float ms = 0;
   cudaEventElapsedTime(&ms, ctx->ev[0], ctx->ev[1]);
   ctx->stats.fill_ms = ms;

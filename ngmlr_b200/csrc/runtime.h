@@ -202,7 +202,7 @@ struct ngmlr_b200_ctx {
   bool spin_sync = false;           // NGMLR_B200_SPIN_SYNC=1: cudaStreamSynchronize (lowest latency, one busy CPU per waiter)
   unsigned long long big_cells = 8ull << 20;  // a problem is "big" from this many cells ...
   int big_width = 768;                        // ... in a corridor at least this wide
-  int n_big = 0;                    // leading problems of the order that get FILL_BIG_TEAM-warp teams
+  int n_big = 0;                    // leading problems of the order that get FILL_BIG_TEAM-warp teams (0: no such launch)
   bool own_stream = true;
   cudaEvent_t ev[8] = {};
   nb::Scoring sc{};
@@ -223,6 +223,12 @@ struct ngmlr_b200_ctx {
   unsigned long long rf_problems = 0;  // problems filled by the ramp-free kernels since the context was created
   unsigned long long rf2_problems = 0; // of those, by the kernel with two rows per lane
   unsigned long long rf2_skew_problems = 0;  // of those, in its skewed schedule
+  // Routing counters since the context was created (ngmlr_b200_debug_fill_counts): problems filled by the
+  // FILL_BIG_TEAM-warp launch, by the ramp-free schedule's concurrent launch of ramped 4-warp teams, by the ordinary
+  // launch's ramped one-warp and ramped 4-warp team kernels, and by the RAW instantiation (whatever the launch); fill
+  // launches, those with more than one of the three concurrent launches non-empty, and those with all three.
+  unsigned long long big_team_problems = 0, rf_team_problems = 0, ramped_warp_problems = 0, ramped_team_problems = 0;
+  unsigned long long raw_problems = 0, fill_launch_count = 0, multi_launch_count = 0, three_way_launch_count = 0;
   int rows_per_lane = 2;  // rows per lane of the ramp-free kernel: 1 or 2 (NGMLR_B200_FILL_ROWS_PER_LANE)
   int rf2_skew = 1;       // two rows per lane: the second row one column behind the first (NGMLR_B200_FILL_RF2_SKEW)
   int rf_team = 0;        // problems after the big ones with >= rf_team_cells cells (they lead the order)
