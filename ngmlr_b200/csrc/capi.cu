@@ -26,21 +26,53 @@ using namespace nb;
 
 std::string g_create_error;
 
-// Scorings for which the as-coded SSE fill (raw indelRun in the run tests) can differ from the
-// scalar rule: a gap-open out of a cell that was itself reached through the *other* gap type
-// would have to tie with or beat the diagonal. Sufficient condition for equivalence, with a
-// margin far above float rounding at alignment-score magnitudes:
-//   open < 0 and max(open, ext_min) + open <= min(match, mismatch) - 0.25   (both gap kinds)
-// Default scoring (2,-5,-5,-5,-1,0.15): -6 <= -5.25 -> scalar kernel. Otherwise the RAW kernel.
-bool scoring_needs_raw(const Scoring& s) {
+}  // namespace
+
+namespace nb {
+
+// When may a batch take the scalar-rule kernel? The as-coded SSE fill (raw indelRun in the run tests) and the
+// scalar rule differ only where a gap-open out of a cell that was itself reached through the *other* gap type ties
+// with or beats the diagonal. Take an insertion opened below a deletion cell: with S = S(x-1, y-1),
+//   U  = fl(fl(S + p) + open)   (p <= max(open, ext_min): the deletion's open or convex extension)
+//   dg = fl(S + sub)            (sub >= min(match, mismatch))
+// (the deletion opened right of an insertion cell is the same with the roles swapped). Exactly, U <= dg - margin with
+//   margin = min(match, mismatch) - max(max(open, ext_min) + open)   (both gap kinds),
+// and the three roundings move U - dg by at most 1.5 ulp(M), M a bound on the magnitude of S + max(p, 0) and dg.
+// So U < dg, and the scalar rule equals the SSE fill, when open < 0 and margin > 1.5 ulp(M). The margin is an
+// absolute number while ulp(M) grows with the scores: at (512,-64,-32.125,-32.125,-32.125,0.5) (margin 0.25, every
+// option in ngmlr's CLI range) a 9 kb read scores ~4 M, where 1.5 ulp = 0.375, and the two rules do give different
+// alignments (tests/test_scoring_oracle.py).
+// The class test keeps its float form and 0.25 floor (what the oracle and the reference have been compared on); the
+// magnitude test takes M from score_magnitude_bound() of the batch's largest problem. Default scoring
+// (2,-5,-5,-5,-1,0.15), margin 1: scalar kernel until M reaches 2^23, i.e. reads and windows of about 2.9 M bases.
+bool scoring_needs_raw(const Scoring& s, double magnitude) {
   const float sub_min = std::min(s.mat, s.mis);
-  const bool ok = s.open_read < 0.0f && s.open_ref < 0.0f &&
-                  std::max(s.open_ref, s.ext_min) + s.open_read <= sub_min - 0.25f &&
-                  std::max(s.open_read, s.ext_min) + s.open_ref <= sub_min - 0.25f;
-  return !ok;
+  const bool in_class = s.open_read < 0.0f && s.open_ref < 0.0f &&
+                        std::max(s.open_ref, s.ext_min) + s.open_read <= sub_min - 0.25f &&
+                        std::max(s.open_read, s.ext_min) + s.open_ref <= sub_min - 0.25f;
+  if (!in_class) return true;
+  const double margin = (double)sub_min - std::max((double)std::max(s.open_ref, s.ext_min) + (double)s.open_read,
+                                                   (double)std::max(s.open_read, s.ext_min) + (double)s.open_ref);
+  int e = 0;
+  std::frexp(magnitude, &e);  // magnitude in [2^(e-1), 2^e): float ulp 2^(e-24)
+  const double ulp = magnitude > 0.0 ? std::ldexp(1.0, e - 24) : 0.0;
+  return !(margin > 1.5 * ulp);
 }
 
-}  // namespace
+// Bound on the magnitude M above for one problem. A path to any cell takes at most min(qryLen, refLen) diagonal
+// steps, each adding <= max(match, mismatch, 0), and at most qryLen + refLen gap steps, each adding <= max(open,
+// ext_min, 0) (positive only through the C ABI); S is never below 0. Each of those <= qryLen + refLen float
+// additions rounds by at most 2^-24 relative, which the last factor, exp(steps 2^-24) >= (1 + 2^-24)^steps, covers. Then S + max(p, 0) and |dg| add one gap
+// and one substitution score.
+double score_magnitude_bound(const Scoring& s, long long qry_len, long long ref_len) {
+  const double gain = std::max({(double)s.mat, (double)s.mis, 0.0});
+  const double gap = std::max({(double)s.open_read, (double)s.open_ref, (double)s.ext_min, 0.0});
+  const double steps = (double)(qry_len + ref_len);
+  const double smax = (gain * (double)std::min(qry_len, ref_len) + gap * steps) * std::exp(steps * 0x1p-24);
+  return smax + gap + std::max(std::fabs((double)s.mat), std::fabs((double)s.mis));
+}
+
+}  // namespace nb
 
 void nb_cs_release(ngmlr_b200_ctx* ctx);  // candidate-search state lives in a side table (below)
 
@@ -119,7 +151,6 @@ int ngmlr_b200_create(int gpu_id, const ngmlr_b200_scoring* s, ngmlr_b200_ctx** 
   ctx->sc.gap_ext = d.gap_extend;
   ctx->sc.ext_min = d.gap_extend_min;
   ctx->sc.decay = d.gap_decay;
-  ctx->raw = scoring_needs_raw(ctx->sc);
   if (const char* e = getenv("NGMLR_B200_FILL_TEAM")) ctx->force_team = atoi(e);
   if (const char* e = getenv("NGMLR_B200_FILL_SCHEDULE")) {
     if (!strcmp(e, "ramped")) ctx->fill_schedule = 0;

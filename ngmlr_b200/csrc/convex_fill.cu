@@ -36,7 +36,8 @@
 // direction priority is the reference's. `RAW` selects the as-coded SSE semantics in which the
 // run tests use the neighbours' raw indelRun for all but the last <=12 cells of a row (executable
 // spec: oracle/convex_oracle.c chain_cell, rule 2); RAW=false is the scalar rule, which is
-// identical for every scoring in the "default class" (see capi.cu scoring_needs_raw()).
+// identical for every scoring in the "default class" up to the score magnitude where float rounding can erase the
+// class's margin (see capi.cu scoring_needs_raw(), chosen per batch).
 #include <cuda_runtime.h>
 #include <limits.h>
 

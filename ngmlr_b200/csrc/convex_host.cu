@@ -194,7 +194,9 @@ int convex_upload_spec(ngmlr_b200_ctx* ctx, const UploadSpec& sp) {
   ctx->team_safe = true;
   ctx->rf_wide = 0;
   ctx->rf_fits = true;
+  double magnitude = 0.0;  // bound on the scores of the batch: the scalar-rule kernel is exact below it (capi.cu)
   for (int i = 0; i < n; ++i) {
+    magnitude = std::max(magnitude, score_magnitude_bound(ctx->sc, qry_lens[i], ref_lens[i]));
     // The ramp-free kernel numbers the steps of a problem in an int: a block adds at most its column span
     // (<= refLen + 1) plus the hand-off and placement slack (< 400 steps) -- keep the total below 2^30.
     if ((((long long)qry_lens[i] + 31) / 32) * ((long long)ref_lens[i] + 400) >= (1ll << 30)) ctx->rf_fits = false;
@@ -210,6 +212,7 @@ int convex_upload_spec(ngmlr_b200_ctx* ctx, const UploadSpec& sp) {
     ctx->ext_qs[i] = ctx->h_desc.p[i].ext_qstart;
     ctx->ext_qe[i] = ctx->h_desc.p[i].ext_qend;
   }
+  ctx->raw = scoring_needs_raw(ctx->sc, magnitude);
   const size_t so = seq_bytes, bo = nblocks;
   // Largest first (LPT); the few huge and wide matrices of a batch -- realignments, full matrices, corridors
   // widened by the anchors around a long indel -- lead the order: they get FILL_BIG_TEAM-warp teams.

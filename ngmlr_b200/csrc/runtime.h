@@ -206,7 +206,7 @@ struct ngmlr_b200_ctx {
   bool own_stream = true;
   cudaEvent_t ev[8] = {};
   nb::Scoring sc{};
-  bool raw = false;
+  bool raw = false;  // the batch needs the RAW fill kernel: its scoring, at the magnitude its problems can reach
   int force_raw = -1;
   std::string error;
 
@@ -440,5 +440,10 @@ struct CsState {
 CsState* cs_state(ngmlr_b200_ctx* ctx, bool create);
 
 int convex_upload_spec(ngmlr_b200_ctx* ctx, const UploadSpec& spec);
+
+// Fill kernel choice (capi.cu): whether a batch under scoring `s` whose scores stay below `magnitude` needs the RAW
+// (as-coded SSE) kernel, and the magnitude bound of one problem.
+bool scoring_needs_raw(const Scoring& s, double magnitude);
+double score_magnitude_bound(const Scoring& s, long long qry_len, long long ref_len);
 
 }  // namespace nb
