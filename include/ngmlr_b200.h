@@ -512,14 +512,17 @@ int ngmlr_b200_dedupe_short_read_candidates(int n, const int64_t* cand_start, co
                                             int read_part_length, int32_t* kept, int64_t* kept_start);
 
 /* scoreShortRead's scores (src/ScoreBuffer.cpp:245-272) for n (resident read, location, strand) pairs: read
- * read_index[i] of ngmlr_b200_reads_upload (at most 256 bases), or its MappedRead::computeReverseSeq when
+ * read_index[i] of ngmlr_b200_reads_upload (any resident read), or its MappedRead::computeReverseSeq when
  * reverse[i], against DecodeRefSequence(buf, 0, loc - (corridor >> 1), len + corridor) with
- * corridor = (int)(len * 0.3 + 256) ('N' x (len + corridor) where decoding fails), StrippedSW::SingleScore semantics.
- * Windows decoded straight from the resident genome on the device. Returns n or < 0. */
+ * corridor = (int)(len * 0.3 + 256) ('N' x (len + corridor) where decoding fails), StrippedSW::SingleScore semantics
+ * (-1 for a read or window of >= 100000 characters). Windows decoded straight from the resident genome on the
+ * device. Reads of at most 510 bases are scored by the packed ungapped path (exact for them: a gap costs 255); longer
+ * ones by the general affine path. Returns n or < 0. */
 int ngmlr_b200_score_short_reads(ngmlr_b200_ctx* ctx, int n, const int32_t* read_index, const uint64_t* locs,
                                  const uint8_t* reverse, float* scores);
 
-/* The whole short-read path for every read of the resident batch of at most read_part_length (<= 256) bases, after
+/* The whole short-read path for every read of the resident batch of at most read_part_length (>= 1, no upper limit)
+ * bases, after
  * ngmlr_b200_reads_upload (same read_part_length) + ngmlr_b200_cs_run: duplicate removal, scoring as
  * ngmlr_b200_score_short_reads, order + MQ as ngmlr_b200_select_candidates (without the 0.75 cut), the alignment loop
  * of processShortRead (src/AlignmentBuffer.cpp:2564-2639; each candidate aligned as computeAlignment(..., shortRead =

@@ -167,6 +167,9 @@ def load():
                                                  C.POINTER(C.c_float)]
     lib.ngmlr_b200_debug_short_read_general_pairs.argtypes = [vp]
     lib.ngmlr_b200_debug_short_read_general_pairs.restype = C.c_uint
+    for name in ("short_read_wide_pairs", "subread_general_pairs", "subread_wide_pairs"):
+        getattr(lib, "ngmlr_b200_debug_" + name).argtypes = [vp]
+        getattr(lib, "ngmlr_b200_debug_" + name).restype = C.c_uint
     # the records' type is samtext.SamAln (passed as an untyped pointer here: samtext imports this module)
     lib.ngmlr_b200_map_short_reads.argtypes = [vp, C.c_int, C.c_float, i32p, i64p, i32p, C.POINTER(vp), i64p]
     lib.ngmlr_b200_load_reference.argtypes = [vp, C.c_char_p, C.POINTER(ReferenceOptions), i32p, u64p, i32p]

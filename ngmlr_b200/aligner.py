@@ -595,6 +595,17 @@ class B200Aligner:
         """Test hook: of those, problems filled with the second row of each lane one column behind its first."""
         return int(self.lib.ngmlr_b200_debug_rampfree2_skew_problems(self.h))
 
+    def debug_short_read_pairs(self):
+        """Test hook: pairs of the last short-read scoring (score_short_reads, map_short_reads) by scorer branch --
+        the general affine path (general) and the ungapped path of the wide instantiation (wide)."""
+        return {"general": int(self.lib.ngmlr_b200_debug_short_read_general_pairs(self.h)),
+                "wide": int(self.lib.ngmlr_b200_debug_short_read_wide_pairs(self.h))}
+
+    def debug_subread_pairs(self):
+        """Test hook: the same counters for the last sub-read scoring (cs_run, cs_score)."""
+        return {"general": int(self.lib.ngmlr_b200_debug_subread_general_pairs(self.h)),
+                "wide": int(self.lib.ngmlr_b200_debug_subread_wide_pairs(self.h))}
+
     FILL_COUNTS = ("big_team", "rf_team", "rampfree", "ramped_warp", "ramped_team", "raw",
                    "fill_launches", "multi_launch", "three_way")
 

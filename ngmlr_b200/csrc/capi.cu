@@ -481,6 +481,7 @@ int ngmlr_b200_sw_score_batch(ngmlr_b200_ctx* ctx, int n, const char* const* ref
   CU(cudaMemcpyAsync(ctx->d_sw_off.p, ctx->h_sw_off.p, (size_t)2 * n * sizeof(uint64_t), cudaMemcpyHostToDevice, st));
   CU(cudaMemcpyAsync(ctx->d_sw_len.p, ctx->h_sw_len.p, (size_t)2 * n * sizeof(int32_t), cudaMemcpyHostToDevice, st));
   SwParams sp;
+  memset(&sp, 0, sizeof(sp));
   sp.seq = ctx->d_sw_seq.p;
   sp.ref_off = ctx->d_sw_off.p;
   sp.qry_off = ctx->d_sw_off.p + n;
@@ -491,7 +492,7 @@ int ngmlr_b200_sw_score_batch(ngmlr_b200_ctx* ctx, int n, const char* const* ref
   sp.scratch = ctx->d_sw_scratch.p;
   sp.scratch_stride = stride;
   CU(cudaEventRecord(ctx->ev[4], st));
-  CU(launch_sw_score(sp, grid, st));
+  CU(launch_sw_score(sp, grid, max_qry, max_ref - 1, st));
   CU(cudaEventRecord(ctx->ev[5], st));
   CU(cudaMemcpyAsync(ctx->h_sw_out.p, ctx->d_sw_out.p, (size_t)n * sizeof(float), cudaMemcpyDeviceToHost, st));
   CU(nb_stream_sync(ctx, st));
@@ -746,9 +747,11 @@ int ngmlr_b200_cs_search_batch(ngmlr_b200_ctx* ctx, int n, const char* const* se
   // ---- reads -> device ----
   std::vector<uint64_t> seq_off(n);
   size_t bytes = 0;
+  int max_len = 0;
   for (int i = 0; i < n; ++i) {
     seq_off[i] = bytes;
     bytes += align_up((size_t)std::max(lens[i], 0) + 1, 16);
+    max_len = std::max(max_len, lens[i]);
   }
   cs->last_seq_off = seq_off;
   cs->rn = 0;              // d_seq / d_off / d_len are shared with the resident pipeline: invalidate it
@@ -1133,7 +1136,11 @@ int ngmlr_b200_cs_score_batch(ngmlr_b200_ctx* ctx, int n, const char* const* seq
   sp.win_pos = cs->d_winpos.p;
   sp.rev = cs->d_rev.p;
   sp.win_len = win_len;
-  CU(launch_sw_score_gather(sp, grid, st));
+  CU(cs->d_sub_counts.reserve(2));
+  CU(cudaMemsetAsync(cs->d_sub_counts.p, 0, 2 * sizeof(unsigned int), st));
+  sp.general_pairs = cs->d_sub_counts.p;
+  sp.wide_pairs = cs->d_sub_counts.p + 1;
+  CU(launch_sw_score_gather(sp, grid, max_q, win_len, st));
   CU(cudaMemcpyAsync(cs->sw_scores.data(), cs->d_sw.p, m * 4, cudaMemcpyDeviceToHost, st));
   CU(nb_stream_sync(ctx, st));
   return rc;
@@ -1151,9 +1158,11 @@ int ngmlr_b200_cs_upload(ngmlr_b200_ctx* ctx, int n, const char* const* seqs, co
   cudaStream_t st = ctx->stream;
   std::vector<uint64_t> seq_off((size_t)n + 1);
   size_t bytes = 0;
+  int max_len = 0;
   for (int i = 0; i < n; ++i) {
     seq_off[i] = bytes;
     bytes += align_up((size_t)std::max(lens[i], 0) + 1, 16);
+    max_len = std::max(max_len, lens[i]);
   }
   CU(cs->p_seq.reserve(bytes + 16));
   uint8_t* hseq = cs->p_seq.p;
@@ -1172,6 +1181,7 @@ int ngmlr_b200_cs_upload(ngmlr_b200_ctx* ctx, int n, const char* const* seqs, co
   }
   CU(nb_stream_sync(ctx, st));
   cs->rn = n;
+  cs->rmax = max_len;
   cs->rbytes = bytes;
   cs->seq_base = cs->d_seq.p;
   cs->n_cand = 0;
@@ -1280,6 +1290,8 @@ int ngmlr_b200_cs_run(ngmlr_b200_ctx* ctx, float sensitivity, float min_kmer_hit
   CU(launch_cs_compact(cs->d_out.p, reinterpret_cast<const uint64_t*>(cs->d_sc.p), cs->d_count.p, cs->d_cstart.p,
                        cs->d_off.p, cs->d_len.p, n, corridor >> 1, cs->d_cloc.p, cs->d_cscore.p, cs->d_rev.p,
                        cs->d_winpos.p, cs->d_qoff.p, cs->d_qlen.p, st));
+  CU(cs->d_sub_counts.reserve(2));
+  CU(cudaMemsetAsync(cs->d_sub_counts.p, 0, 2 * sizeof(unsigned int), st));
   if (m) {
     const int win_len = ((read_part_length + 10 + corridor) | 1) + 1;  // refMaxLen, src/ScoreBuffer.h:71-72
     const int warps_per_cta = 4;
@@ -1302,7 +1314,9 @@ int ngmlr_b200_cs_run(ngmlr_b200_ctx* ctx, float sensitivity, float min_kmer_hit
     sp.win_pos = cs->d_winpos.p;
     sp.rev = cs->d_rev.p;
     sp.win_len = win_len;
-    CU(launch_sw_score_gather(sp, grid, st));
+    sp.general_pairs = cs->d_sub_counts.p;
+    sp.wide_pairs = cs->d_sub_counts.p + 1;
+    CU(launch_sw_score_gather(sp, grid, cs->rmax + 1, win_len, st));
   }
   CU(cudaEventRecord(cs->ev1, st));
   CU(nb_stream_sync(ctx, st));
@@ -1311,6 +1325,22 @@ int ngmlr_b200_cs_run(ngmlr_b200_ctx* ctx, float sensitivity, float min_kmer_hit
   if (kernel_ms) cudaEventElapsedTime(kernel_ms, cs->ev0, cs->ev1);
   return 0;
 }
+
+// Test-only counters of the last sub-read scoring launch (cs_run or cs_score_batch): pairs that took the general
+// path, and pairs that took the ungapped path of the wide instantiation.
+static unsigned int subread_count(ngmlr_b200_ctx* ctx, int which) {
+  CsState* cs = ctx ? cs_state(ctx, false) : nullptr;
+  unsigned int v[2] = {0u, 0u};
+  if (!cs || !cs->d_sub_counts.p) return 0u;
+  if (cudaSetDevice(ctx->device) != cudaSuccess || cudaStreamSynchronize(ctx->stream) != cudaSuccess ||
+      cudaMemcpy(v, cs->d_sub_counts.p, sizeof(v), cudaMemcpyDeviceToHost) != cudaSuccess)
+    return 0u;
+  return v[which];
+}
+
+unsigned int ngmlr_b200_debug_subread_general_pairs(ngmlr_b200_ctx* ctx) { return subread_count(ctx, 0); }
+
+unsigned int ngmlr_b200_debug_subread_wide_pairs(ngmlr_b200_ctx* ctx) { return subread_count(ctx, 1); }
 
 int ngmlr_b200_cs_fetch(ngmlr_b200_ctx* ctx, int64_t* cand_start, const float** cs_scores,
                         const uint64_t** locs, const uint8_t** reverse, const float** sw_scores,

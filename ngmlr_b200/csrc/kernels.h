@@ -72,12 +72,19 @@ struct SwParams {
   int win_len;                 // refMaxLen (308)
   // short-read scoring (ScoreBuffer::scoreShortRead): the window length of pair i is win_lens[i]
   const int32_t* win_lens;
-  unsigned int* general_pairs; // optional: counts pairs of the short-read launch that miss the ungapped path
+  unsigned int* general_pairs; // optional: counts pairs that miss the ungapped path (general affine path)
+  unsigned int* wide_pairs;    // optional: counts pairs of the ungapped path in the wide instantiation
 };
-cudaError_t launch_sw_score(const SwParams& p, int grid, cudaStream_t stream);
-cudaError_t launch_sw_score_gather(const SwParams& p, int grid, cudaStream_t stream);
-// gather mode with per-pair windows of up to 640 columns (short reads: len + (int)(len * 0.3 + 256) <= 588)
-cudaError_t launch_sw_score_gather_short(const SwParams& p, int grid, cudaStream_t stream);
+// Each launch picks its instantiation from the batch's longest query (max_qry_len, NUL included) and widest window
+// (max_cols: ref / window characters, NUL excluded): the default one (queries of <= 320 rows, windows of <= 384
+// columns; 640 for the short-read launch) when both fit, else the wide one (ungapped up to 510 rows and 1024
+// columns). Pairs outside the ungapped path take the general path in either; scratch_stride must then hold the
+// widest window + 1 whenever a query is longer than 288 characters (multi-pass).
+cudaError_t launch_sw_score(const SwParams& p, int grid, int max_qry_len, int max_cols, cudaStream_t stream);
+cudaError_t launch_sw_score_gather(const SwParams& p, int grid, int max_qry_len, int max_cols, cudaStream_t stream);
+// gather mode with per-pair windows (p.win_lens; short reads: len + (int)(len * 0.3 + 256) columns)
+cudaError_t launch_sw_score_gather_short(const SwParams& p, int grid, int max_qry_len, int max_cols,
+                                         cudaStream_t stream);
 
 cudaError_t launch_decode_windows(const RefDecodeParams& p, cudaStream_t stream);
 // one contig's characters (device) -> 4-bit codes, two per byte (_SequenceProvider::Init's encoding)

@@ -203,12 +203,14 @@ int ngmlr_b200_reads_upload(ngmlr_b200_ctx* ctx, int n_reads, const char* const*
   ctx->read_off.resize((size_t)n_reads + 1);
   ctx->read_len.assign(lens, lens + n_reads);
   size_t bytes = 0, n_sub = 0;
+  int max_sub = 0;  // the longest sub-read
   for (int i = 0; i < n_reads; ++i) {
     if (lens[i] < 0) return ctx->fail("reads_upload: negative length at %d", i);
     ctx->read_off[i] = bytes;
     bytes += align_up((size_t)lens[i] + 1, 16);
     const int parts = lens[i] / read_part_length;
     n_sub += parts > 0 ? (size_t)parts : 1;  // a read shorter than one part is its own sub-read (:76-104)
+    max_sub = std::max(max_sub, parts > 0 ? read_part_length : lens[i]);
   }
   ctx->read_off[n_reads] = bytes;
   if (n_sub > 0x7fffffffull) return ctx->fail("reads_upload: too many sub-reads");
@@ -253,6 +255,7 @@ int ngmlr_b200_reads_upload(ngmlr_b200_ctx* ctx, int n_reads, const char* const*
   ctx->reads_bytes = bytes;
   // stage 0/2 now runs on the sub-reads of the resident set (ngmlr_b200_cs_run / cs_fetch)
   cs->rn = (int)n_sub;
+  cs->rmax = max_sub;
   cs->rbytes = bytes;
   cs->seq_base = ctx->d_reads.p;
   cs->n_cand = 0;

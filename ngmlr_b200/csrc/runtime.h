@@ -406,6 +406,7 @@ struct CsState {
   std::vector<uint64_t> last_seq_off;  // arena offsets of the reads of the last search
   // resident pipeline
   int rn = 0;                       // (sub-)reads the resident pipeline runs on
+  int rmax = 0;                     // the longest of them
   size_t rbytes = 0;
   const uint8_t* seq_base = nullptr;  // their arena: d_seq (cs_upload) or the context's resident read set
   DevBuf<unsigned long long> d_a, d_b, d_c, d_sa, d_sb, d_sc, d_cnt64, d_cstart, d_cloc;
@@ -426,9 +427,11 @@ struct CsState {
   DevBuf<uint64_t> d_sr_qoff;
   DevBuf<uint8_t> d_sr_rev;
   DevBuf<float> d_sr_sw;
-  DevBuf<unsigned int> d_sr_general;
+  DevBuf<unsigned int> d_sr_counts;  // general pairs | wide ungapped pairs
   DevBuf<int32_t> d_sr_scratch;
   unsigned int sr_general_pairs = 0;  // pairs of the last short-read scoring that missed the ungapped path
+  unsigned int sr_wide_pairs = 0;     // pairs of the last short-read scoring on the wide ungapped instantiation
+  DevBuf<unsigned int> d_sub_counts;  // the same two counters for the last sub-read scoring (cs_run, cs_score_batch)
   // the contig table of the last ngmlr_b200_load_reference (reference_load.cu); cleared when another call replaces
   // the reference
   std::vector<std::string> contig_names;

@@ -8,7 +8,8 @@
 // then aligns the best candidates one by one and hands the read to WriteRead (:3470-3482), which converts the
 // positions to contig coordinates. Here:
 //   dedupe        host (the reference's std::sort of equal locations decides which strand survives)
-//   scoring       device: per-pair window geometry + the StrippedSW kernel's ungapped path (<= 640 columns)
+//   scoring       device: per-pair window geometry + the StrippedSW kernel (ungapped path for reads of <= 510
+//                 bases, the general affine path for longer ones)
 //   order + MQ    host, ngmlr_b200_select_candidates
 //   align loop    rounds: round r aligns candidate r of every read still in its loop, one
 //                 ngmlr_b200_compute_alignments call (short_read = 1) per round
@@ -29,22 +30,30 @@ int score_pairs(ngmlr_b200_ctx* ctx, CsState* cs, int n, const int32_t* read_ind
                 const uint8_t* reverse, float* scores) {
   cudaStream_t st = ctx->stream;
   cs->sr_general_pairs = 0;
+  cs->sr_wide_pairs = 0;
   if (n == 0) return 0;
+  // the longest query and window of the batch pick the scorer's instantiation and size the general path's strip
+  int max_len = 0;
+  for (int i = 0; i < n; ++i) max_len = std::max(max_len, ctx->read_len[read_index[i]]);
+  max_len = std::min(max_len, 100000);  // longer queries score -1 (maxSeqLen) and need neither
+  const int max_win = max_len + (int)(max_len * 0.3 + 256);  // the longest read has the widest window
   const size_t nn = (size_t)n + 1;
   CU(cs->d_sr_ridx.reserve(nn)); CU(cs->d_sr_winlen.reserve(nn)); CU(cs->d_sr_qlen.reserve(nn));
   CU(cs->d_sr_loc.reserve(nn)); CU(cs->d_sr_winpos.reserve(nn)); CU(cs->d_sr_qoff.reserve(nn));
-  CU(cs->d_sr_rev.reserve(nn)); CU(cs->d_sr_sw.reserve(nn)); CU(cs->d_sr_general.reserve(1));
+  CU(cs->d_sr_rev.reserve(nn)); CU(cs->d_sr_sw.reserve(nn)); CU(cs->d_sr_counts.reserve(2));
   CU(ctx->d_read_len.reserve((size_t)ctx->n_reads + 1));
   CU(cudaMemcpyAsync(ctx->d_read_len.p, ctx->read_len.data(), (size_t)ctx->n_reads * 4, cudaMemcpyHostToDevice, st));
   CU(cudaMemcpyAsync(cs->d_sr_ridx.p, read_index, (size_t)n * 4, cudaMemcpyHostToDevice, st));
   CU(cudaMemcpyAsync(cs->d_sr_loc.p, locs, (size_t)n * 8, cudaMemcpyHostToDevice, st));
   CU(cudaMemcpyAsync(cs->d_sr_rev.p, reverse, (size_t)n, cudaMemcpyHostToDevice, st));
-  CU(cudaMemsetAsync(cs->d_sr_general.p, 0, sizeof(unsigned int), st));
+  CU(cudaMemsetAsync(cs->d_sr_counts.p, 0, 2 * sizeof(unsigned int), st));
   CU(launch_cs_short_geometry(cs->d_sr_ridx.p, cs->d_sr_loc.p, ctx->d_read_off.p, ctx->d_read_len.p, n,
                               cs->d_sr_winpos.p, cs->d_sr_winlen.p, cs->d_sr_qoff.p, cs->d_sr_qlen.p, st));
   const int warps_per_cta = 4;
   const int grid = std::max(1, std::min(ctx->num_sms * 8, (n + warps_per_cta - 1) / warps_per_cta));
-  const size_t stride = 4;  // queries of <= 257 characters never reach the multi-pass strip
+  // queries of more than 288 characters take several passes of the general path, carried by a strip of one int2
+  // per window column (the NUL included)
+  const size_t stride = max_len + 1 > 288 ? align_up((size_t)max_win + 4, 4) : 4;
   CU(cs->d_sr_scratch.reserve((size_t)grid * warps_per_cta * stride * 2));
   SwParams sp;
   memset(&sp, 0, sizeof(sp));
@@ -60,11 +69,15 @@ int score_pairs(ngmlr_b200_ctx* ctx, CsState* cs, int n, const int32_t* read_ind
   sp.win_pos = cs->d_sr_winpos.p;
   sp.rev = cs->d_sr_rev.p;
   sp.win_lens = cs->d_sr_winlen.p;
-  sp.general_pairs = cs->d_sr_general.p;
-  CU(launch_sw_score_gather_short(sp, grid, st));
+  sp.general_pairs = cs->d_sr_counts.p;
+  sp.wide_pairs = cs->d_sr_counts.p + 1;
+  CU(launch_sw_score_gather_short(sp, grid, max_len + 1, max_win, st));
   CU(cudaMemcpyAsync(scores, cs->d_sr_sw.p, (size_t)n * 4, cudaMemcpyDeviceToHost, st));
-  CU(cudaMemcpyAsync(&cs->sr_general_pairs, cs->d_sr_general.p, sizeof(unsigned int), cudaMemcpyDeviceToHost, st));
+  unsigned int counts[2] = {0u, 0u};
+  CU(cudaMemcpyAsync(counts, cs->d_sr_counts.p, sizeof(counts), cudaMemcpyDeviceToHost, st));
   CU(nb_stream_sync(ctx, st));
+  cs->sr_general_pairs = counts[0];
+  cs->sr_wide_pairs = counts[1];
   return 0;
 }
 
@@ -134,8 +147,6 @@ int ngmlr_b200_score_short_reads(ngmlr_b200_ctx* ctx, int n, const int32_t* read
   for (int i = 0; i < n; ++i) {
     if (read_index[i] < 0 || read_index[i] >= ctx->n_reads)
       return ctx->fail("score_short_reads: read index out of range at %d", i);
-    if (ctx->read_len[read_index[i]] > 256)
-      return ctx->fail("score_short_reads: read %d is longer than 256 bases", read_index[i]);
   }
   CU(cudaSetDevice(ctx->device));
   if (score_pairs(ctx, cs, n, read_index, locs, reverse, scores)) return -1;
@@ -147,13 +158,17 @@ unsigned int ngmlr_b200_debug_short_read_general_pairs(ngmlr_b200_ctx* ctx) {
   return cs ? cs->sr_general_pairs : 0u;
 }
 
+unsigned int ngmlr_b200_debug_short_read_wide_pairs(ngmlr_b200_ctx* ctx) {
+  CsState* cs = ctx ? cs_state(ctx, false) : nullptr;
+  return cs ? cs->sr_wide_pairs : 0u;
+}
+
 int ngmlr_b200_map_short_reads(ngmlr_b200_ctx* ctx, int read_part_length, float min_residues, int32_t* n_aln,
                                int64_t* first_aln, int32_t* mapped, const ngmlr_b200_sam_aln** alns,
                                int64_t* n_alns_total) {
   if (!ctx) return -1;
   if (!n_aln || !first_aln || !mapped || !alns || !n_alns_total) return ctx->fail("map_short_reads: NULL output");
-  if (read_part_length < 1 || read_part_length > 256)
-    return ctx->fail("map_short_reads: read_part_length must be in 1 .. 256");
+  if (read_part_length < 1) return ctx->fail("map_short_reads: read_part_length < 1");
   CsState* cs = cs_state(ctx, false);
   if (check_short_ready(ctx, cs, "map_short_reads")) return -1;
   if (!cs->reads_searched) return ctx->fail("map_short_reads: call cs_run on the uploaded reads first");

@@ -12,10 +12,12 @@
 //     saturating subtraction (clamp at 0); result = max H as uint16 -> float.
 //
 // Mapping: one warp per pair; the warp sweeps the reference columns as a wavefront (lane t is one
-// column behind lane t-1). The hot case (256-bp sub-read against a ~306-bp window) is provably
-// ungapped and runs in sw_ungapped() below: packed 16-bit rows, substitution scores by PRMT table
-// lookup, ~2 instructions per cell. Everything else takes the general affine path: lane t owns
-// SW_ROWS consecutive query rows and passes the H and F of its last row down with __shfl_up;
+// column behind lane t-1). Every pair with a query of at most 511 characters (NUL included) is
+// provably ungapped; when its window fits the instantiation's shared table (the hot case: 256-bp
+// sub-read against a ~306-bp window) it runs in sw_ungapped() below: packed 16-bit rows,
+// substitution scores by PRMT table lookup, ~2 instructions per 2 cells. Everything else takes the
+// general affine path: lane t owns SW_ROWS consecutive query rows and passes the H and F of its
+// last row down with __shfl_up;
 // queries longer than 32*SW_ROWS rows are processed in several passes, the bottom row of a pass is
 // carried to the next through a per-warp strip in global memory; 32-bit integer lanes emulate the
 // int16 saturation (values never exceed 32767).
@@ -35,6 +37,15 @@ constexpr int SW_COLS = 384;  // widest window of the ungapped hot path (ScoreBu
 // widest window of the short-read scorer's instantiation: scoreShortRead's windows have
 // len + (int)(len * 0.3 + 256) <= 588 characters for reads of <= 256 bases
 constexpr int SW_COLS_SHORT = 640;
+// The default instantiations above keep rows per lane at <= 2 * 5 (queries of <= 320 rows): their register count
+// and shared-memory footprint are what the default workload runs at. The wide instantiation takes every other
+// pair the ungapped path is exact for: up to 2 * 8 rows per lane (510 rows) and windows of up to 1024 columns --
+// short reads of <= 510 bases (<= 510 + 409 = 919 columns) and sub-read windows at --subread-length <= 510.
+constexpr int SW_PAIRS_DEFAULT = 5;
+constexpr int SW_PAIRS_WIDE = 8;
+constexpr int SW_COLS_WIDE = 1024;
+// The ungapped path is exact for at most 510 query rows (511 characters with the NUL), see sw_score_kernel.
+constexpr int SW_UNGAPPED_MAX_ROWS = 510;
 constexpr int SW_WARPS_PER_CTA = 4;
 
 __device__ __forceinline__ int nt_code(uint32_t c) {
@@ -162,9 +173,24 @@ __device__ __forceinline__ float sw_ungapped(const GenomeWindow& gw, const uint8
   return (float)(best & 0xffff);
 }
 
-// COLS: widest window of the ungapped path (shared table size); PAIR_WIN: window lengths per pair (p.win_lens)
-template <bool GATHER, int COLS, bool PAIR_WIN>
+// The narrowest rows-per-lane instantiation (PAIRS = 4 .. MAX_PAIRS) that holds qrows query rows: the step cost
+// grows with PAIRS.
+template <int PAIRS, int MAX_PAIRS, bool GATHER>
+__device__ __forceinline__ float sw_ungapped_rows(const GenomeWindow& gw, const uint8_t* __restrict__ ref,
+                                                  const uint8_t* __restrict__ qry, int qrows, int cols, bool q_rev,
+                                                  uint32_t* tab, int lane, uint32_t zero) {
+  if constexpr (PAIRS < MAX_PAIRS) {
+    if (qrows > 64 * PAIRS)
+      return sw_ungapped_rows<PAIRS + 1, MAX_PAIRS, GATHER>(gw, ref, qry, qrows, cols, q_rev, tab, lane, zero);
+  }
+  return sw_ungapped<PAIRS, GATHER>(gw, ref, qry, qrows, cols, q_rev, tab, lane, zero);
+}
+
+// COLS: widest window of the ungapped path (shared table size); MAX_PAIRS: most rows per lane of the ungapped path
+// (2 * MAX_PAIRS); PAIR_WIN: window lengths per pair (p.win_lens)
+template <bool GATHER, int COLS, int MAX_PAIRS, bool PAIR_WIN>
 __global__ void __launch_bounds__(SW_WARPS_PER_CTA * 32) sw_score_kernel(const SwParams p) {
+  constexpr int UNGAPPED_ROWS = 64 * MAX_PAIRS < SW_UNGAPPED_MAX_ROWS ? 64 * MAX_PAIRS : SW_UNGAPPED_MAX_ROWS;
   const int lane = threadIdx.x & 31;
   const int warp_global = blockIdx.x * SW_WARPS_PER_CTA + (threadIdx.x >> 5);
   const int nwarps = gridDim.x * SW_WARPS_PER_CTA;
@@ -190,18 +216,23 @@ __global__ void __launch_bounds__(SW_WARPS_PER_CTA * 32) sw_score_kernel(const S
     const uint8_t* __restrict__ ref = GATHER ? p.seq : p.seq + p.ref_off[pair];
     const uint8_t* __restrict__ qry = p.seq + p.qry_off[pair];
     int best = 0;
-    // ---- hot case: at most 320 query characters (256-bp sub-read + NUL), window of <= COLS columns ----
+    // ---- ungapped case: at most UNGAPPED_ROWS query rows (+ the NUL), window of <= COLS columns ----
     // A gap costs 255 per base, so a gapped path beats its best ungapped piece only if it gains
-    // more than 255 before AND after the gap: impossible with fewer than 512 query characters.
+    // more than 255 before AND after the gap: at least 256 + 256 matching query rows, impossible with
+    // at most 511 query characters (510 rows + the NUL, which scores 0).
     // Then E and F never influence the maximum and the recurrence is H = max(0, diag + s).
-    if (qlen - 1 <= 64 * 5 && rlen - 1 <= COLS) {
-      const float r = (qlen - 1 <= 64 * 4)
-                          ? sw_ungapped<4, GATHER>(gw, ref, qry, qlen - 1, rlen - 1, q_rev, s_tab[threadIdx.x >> 5], lane, zero)
-                          : sw_ungapped<5, GATHER>(gw, ref, qry, qlen - 1, rlen - 1, q_rev, s_tab[threadIdx.x >> 5], lane, zero);
-      if (lane == 0) p.out[pair] = r;
+    if (qlen - 1 <= UNGAPPED_ROWS && rlen - 1 <= COLS) {
+      const float r = sw_ungapped_rows<4, MAX_PAIRS, GATHER>(gw, ref, qry, qlen - 1, rlen - 1, q_rev,
+                                                             s_tab[threadIdx.x >> 5], lane, zero);
+      if (lane == 0) {
+        p.out[pair] = r;
+        if (MAX_PAIRS > SW_PAIRS_DEFAULT && p.wide_pairs) atomicAdd(p.wide_pairs, 1u);
+      }
       continue;
     }
-    if (PAIR_WIN && p.general_pairs && lane == 0) atomicAdd(p.general_pairs, 1u);
+    // the host picks a default instantiation only for batches that fit its ungapped path, so only the short-read one
+    // (per-pair windows, as before the wide one existed) and the wide ones count their general pairs
+    if ((PAIR_WIN || MAX_PAIRS > SW_PAIRS_DEFAULT) && p.general_pairs && lane == 0) atomicAdd(p.general_pairs, 1u);
     const int rows_per_pass = 32 * SW_ROWS;
     for (int row_base = 0; row_base < qlen; row_base += rows_per_pass) {
       const bool first_pass = row_base == 0;
@@ -273,22 +304,32 @@ __global__ void __launch_bounds__(SW_WARPS_PER_CTA * 32) sw_score_kernel(const S
 
 }  // namespace
 
-cudaError_t launch_sw_score(const SwParams& p, int grid, cudaStream_t stream) {
+namespace {
+
+// The default instantiation when the batch's longest query and window fit it, else the wide one.
+template <bool GATHER, int COLS, bool PAIR_WIN>
+cudaError_t launch_sw(const SwParams& p, int grid, int max_qry_len, int max_cols, cudaStream_t stream) {
   if (p.n <= 0) return cudaSuccess;
-  sw_score_kernel<false, SW_COLS, false><<<grid, SW_WARPS_PER_CTA * 32, 0, stream>>>(p);
+  if (max_qry_len - 1 <= 64 * SW_PAIRS_DEFAULT && max_cols <= COLS)
+    sw_score_kernel<GATHER, COLS, SW_PAIRS_DEFAULT, PAIR_WIN><<<grid, SW_WARPS_PER_CTA * 32, 0, stream>>>(p);
+  else
+    sw_score_kernel<GATHER, SW_COLS_WIDE, SW_PAIRS_WIDE, PAIR_WIN><<<grid, SW_WARPS_PER_CTA * 32, 0, stream>>>(p);
   return cudaGetLastError();
 }
 
-cudaError_t launch_sw_score_gather(const SwParams& p, int grid, cudaStream_t stream) {
-  if (p.n <= 0) return cudaSuccess;
-  sw_score_kernel<true, SW_COLS, false><<<grid, SW_WARPS_PER_CTA * 32, 0, stream>>>(p);
-  return cudaGetLastError();
+}  // namespace
+
+cudaError_t launch_sw_score(const SwParams& p, int grid, int max_qry_len, int max_cols, cudaStream_t stream) {
+  return launch_sw<false, SW_COLS, false>(p, grid, max_qry_len, max_cols, stream);
 }
 
-cudaError_t launch_sw_score_gather_short(const SwParams& p, int grid, cudaStream_t stream) {
-  if (p.n <= 0) return cudaSuccess;
-  sw_score_kernel<true, SW_COLS_SHORT, true><<<grid, SW_WARPS_PER_CTA * 32, 0, stream>>>(p);
-  return cudaGetLastError();
+cudaError_t launch_sw_score_gather(const SwParams& p, int grid, int max_qry_len, int max_cols, cudaStream_t stream) {
+  return launch_sw<true, SW_COLS, false>(p, grid, max_qry_len, max_cols, stream);
+}
+
+cudaError_t launch_sw_score_gather_short(const SwParams& p, int grid, int max_qry_len, int max_cols,
+                                         cudaStream_t stream) {
+  return launch_sw<true, SW_COLS_SHORT, true>(p, grid, max_qry_len, max_cols, stream);
 }
 
 }  // namespace nb
