@@ -137,14 +137,18 @@ struct LaneState {
 // One cell (x, y) at step s. `st` is the row's state (LaneState or RowState: lL, lRunF / lIsD or lRun / lDir, kS /
 // kStep, rel); dS = S of (x-1, y-1), {nU, nP} = U and run of (x, y-1), r = the column's reference byte, q = the row's
 // read byte. Returns the direction code; {S, U, P} is what the cell below sees as its up neighbour.
-// SEL_DG: pick the score, then add (both scores stay in registers) instead of a predicated second add, which the
-// compiler turns into a constant-bank load at the head of the cell's dependency chain; the same rounding either way.
-template <bool RAW, bool ALL_ACTIVE, bool SEL_DG = false, class Row>
+// TRIM (the skewed two-row kernel, Row = RowState) trims the half-rate ALU work of a cell, with the same results:
+//  - dg: pick the score, then add (both scores stay in registers) instead of a predicated second add, which the
+//    compiler turns into a constant-bank load at the head of the cell's dependency chain; the same rounding either way;
+//  - scalar rule: "the left cell is a deletion" is read as lRunF > 0 instead of a bool carried across steps (which
+//    the compiler packed into a register with a SEL / LOP3 per cell);
+//  - scalar rule: the factor [S != 0] of e below is a saturating multiply (FMA pipe) instead of an FSET (ALU pipe).
+template <bool RAW, bool ALL_ACTIVE, bool TRIM = false, class Row>
 __device__ __forceinline__ uint32_t cell_update(Row& st, const Scoring& sc, const float dS, const float nU,
                                                 const uint32_t nP, const uint32_t r, const uint32_t q, const bool act,
                                                 const int t0rel, const int s, float& S, float& U, uint32_t& P) {
   float dg;
-  if (SEL_DG) {
+  if (TRIM) {
     dg = __fadd_rn(dS, r == q ? sc.mat : sc.mis);
   } else {
     dg = __fadd_rn(dS, sc.mis);
@@ -190,7 +194,10 @@ __device__ __forceinline__ uint32_t cell_update(Row& st, const Scoring& sc, cons
     //   I  <=>  !D && eU && (ur || !eG)
     // with run lengths kept as floats (exact below 2^24; rows are < 32768 wide here).
     const float upRunF = __uint_as_float(nP);
-    const bool lr = st.lIsD, ur = upRunF > 0.0f;  // the left cell's run is > 0 iff it is a deletion
+    bool lr;  // the left cell's run is > 0 iff it is a deletion
+    if constexpr (TRIM) lr = st.lRunF > 0.0f;
+    else lr = st.lIsD;
+    const bool ur = upRunF > 0.0f;
     const bool X = (eU & ur) | eG;  // bitwise on purpose: straight PLOP3s, no short-circuit
     const bool pD = eL & (lr | !X);
     const bool pI = (!pD) & eU & (ur | !eG);
@@ -208,14 +215,18 @@ __device__ __forceinline__ uint32_t cell_update(Row& st, const Scoring& sc, cons
     const float pen = fminf(sc.ext_min, __fadd_rn(sc.gap_ext, __fmul_rn(runF, sc.decay)));
     // e = (S == 0) ? 0 : S + pen  as one exact fused op: S + pen * [S != 0]
     float nz;
-    asm("set.ne.f32.f32 %0, %1, 0f00000000;" : "=f"(nz) : "f"(S));
+    if (TRIM)  // S * 2^127 saturates to 1 for every S >= 2^-127 (S >= 0). A nonzero S is a sum of scoring values and
+               // so at least the smallest of their ulps: exact for every scoring whose nonzero values are >= 2^-103
+      asm("mul.sat.f32 %0, %1, 0f7F000000;" : "=f"(nz) : "f"(S));
+    else
+      asm("set.ne.f32.f32 %0, %1, 0f00000000;" : "=f"(nz) : "f"(S));
     U = __fadd_rn(S, sc.open_read);
     L = __fadd_rn(S, sc.open_ref);
     if (pI) asm volatile("fma.rn.f32 %0, %1, %2, %3;" : "=f"(U) : "f"(pen), "f"(nz), "f"(S));
     if (pD) asm volatile("fma.rn.f32 %0, %1, %2, %3;" : "=f"(L) : "f"(pen), "f"(nz), "f"(S));
     P = __float_as_uint(newI);
     st.lRunF = newD;
-    st.lIsD = pD;
+    if constexpr (!TRIM) st.lIsD = pD;
   }
   st.lL = L;
   if (S > st.kS) {  // strict: first maximum in row-major order (:1165-1170)

@@ -11,9 +11,12 @@ lane-step) per cell, so the figures compare idle work. No GPU is needed.
 --gpu runs `bench.py --profile-only` and the full `bench.py` under each of --settings (default: all of them),
 alternating, and prints the medians and spreads of the fill kernel time and of the headline value, with the card name,
 power limit and SM clock read in the same run. --dump-outputs also writes each setting's bench outputs once.
+--libraries NAME=PATH,... compares builds of the library instead (NGMLR_B200_LIBRARY, default fill settings), e.g. the
+parent commit's build against the working tree's.
 
     python scripts/fill_schedule.py --cpu [--reads 300]
     python scripts/fill_schedule.py --gpu --runs 3 --out DIR [--settings rampfree-rows2,rampfree-rows2-skew]
+    python scripts/fill_schedule.py --gpu --runs 3 --out DIR --libraries old=/path/libngmlr_b200.so,new=ngmlr_b200/libngmlr_b200.so
 """
 import argparse
 import json
@@ -159,10 +162,13 @@ SETTINGS = {"ramped": ("ramped", "1", "0"), "rampfree-rows1": ("rampfree", "1", 
             "rampfree-rows2": ("rampfree", "2", "0"), "rampfree-rows2-skew": ("rampfree", "2", "1")}
 
 
-def bench(setting, extra, steps, warmup, config):
-    schedule, rows, skew = SETTINGS[setting]
-    env = dict(os.environ, NGMLR_B200_FILL_SCHEDULE=schedule, NGMLR_B200_FILL_ROWS_PER_LANE=rows,
-               NGMLR_B200_FILL_RF2_SKEW=skew)
+def bench(setting, extra, steps, warmup, config, libraries=None):
+    if libraries:
+        env = dict(os.environ, NGMLR_B200_LIBRARY=os.path.abspath(libraries[setting]))
+    else:
+        schedule, rows, skew = SETTINGS[setting]
+        env = dict(os.environ, NGMLR_B200_FILL_SCHEDULE=schedule, NGMLR_B200_FILL_ROWS_PER_LANE=rows,
+                   NGMLR_B200_FILL_RF2_SKEW=skew)
     cmd = [sys.executable, os.path.join(ROOT, "bench.py"), "--gpus", "1", "--steps", str(steps),
            "--warmup", str(warmup), "--config", config] + extra
     r = subprocess.run(cmd, env=env, capture_output=True, text=True, cwd=ROOT)
@@ -174,13 +180,15 @@ def bench(setting, extra, steps, warmup, config):
 
 def gpu(args):
     print("card:", smi())
-    settings = args.settings.split(",") if args.settings else list(SETTINGS)
+    libraries = dict(kv.split("=", 1) for kv in args.libraries.split(",")) if args.libraries else None
+    settings = list(libraries) if libraries else (args.settings.split(",") if args.settings else list(SETTINGS))
     res = {k: {"prof": [], "full": []} for k in settings}
     for i in range(args.runs):
         for sched in settings:
             dump = ["--dump-outputs", os.path.join(args.out, "dump", sched)] if args.dump_outputs and i == 0 else []
-            prof = bench(sched, ["--profile-only"], args.steps, args.warmup, args.config) if not args.full_only else None
-            full = bench(sched, dump, args.steps, args.warmup, args.config)
+            prof = (bench(sched, ["--profile-only"], args.steps, args.warmup, args.config, libraries)
+                    if not args.full_only else None)
+            full = bench(sched, dump, args.steps, args.warmup, args.config, libraries)
             res[sched]["prof"].append(prof)
             res[sched]["full"].append(full)
             print(f"run {i} {sched}: fill {full['kernel_ms_per_step']['fill']:.2f} ms/step, value {full['value']:.4f}, "
@@ -197,6 +205,8 @@ def gpu(args):
             summary[sched].update(solo_fill_ms_median=float(np.median(pfill)),
                                   solo_fill_ms_spread=float(pfill.max() - pfill.min()), solo_fill_ms=pfill.tolist())
     pairs = (("ramped", "rampfree-rows1"), ("rampfree-rows1", "rampfree-rows2"), ("rampfree-rows2", "rampfree-rows2-skew"))
+    if libraries:
+        pairs = tuple(zip(settings, settings[1:]))
     for a, b in (ab for ab in pairs if ab[0] in res and ab[1] in res):
         summary[f"fill_change {a} -> {b}"] = summary[b]["fill_ms_median"] / summary[a]["fill_ms_median"] - 1.0
         summary[f"value_change {a} -> {b}"] = summary[b]["value_median"] / summary[a]["value_median"] - 1.0
@@ -220,6 +230,7 @@ def main():
     ap.add_argument("--config", default="pacbio50", help="bench.py --config")
     ap.add_argument("--full-only", action="store_true", help="skip the --profile-only runs")
     ap.add_argument("--dump-outputs", action="store_true", help="bench.py --dump-outputs OUT/dump/SETTING, first run")
+    ap.add_argument("--libraries", default=None, help="NAME=PATH,...: A/B of library builds (NGMLR_B200_LIBRARY)")
     args = ap.parse_args()
     if args.dump_outputs and not args.out:
         ap.error("--dump-outputs needs --out")
