@@ -539,6 +539,41 @@ int ngmlr_b200_map_short_reads(ngmlr_b200_ctx* ctx, int read_part_length, float 
                                int64_t* first_aln, int32_t* mapped, const ngmlr_b200_sam_aln** alns,
                                int64_t* n_alns_total);
 
+/* ---- reads from a FASTA / FASTQ file (plain or gzip): ReadProvider::NextRead -> FastXParser -> kseq_read ->
+ * IParser::copyToRead (src/ReadProvider.cpp:136-187, src/IParser.h:51-117), parsed on the device ------------------
+ * The file is read in chunks of chunk_bytes (0: 256 MiB) into page-locked memory (gzip inflated by zlib on the calling
+ * thread); a chunk too small for one record grows. Each chunk goes to the device once: its line table, the record
+ * structure (kseq's rules, multi-line FASTQ and quality lines starting with '@' / '>' included) and the normalised
+ * bases are computed there. Device memory of a handle stays below 9 x chunk_bytes. No reference counterpart for
+ * the handle itself. */
+typedef struct ngmlr_b200_read_file ngmlr_b200_read_file;
+typedef struct {
+  int64_t chunk_bytes; /* page-locked staging per chunk; 0 = 256 MiB; grows for a larger record */
+} ngmlr_b200_read_file_options;
+/* opts may be NULL. Returns 0, or < 0 (ngmlr_b200_last_error(NULL) describes it). */
+int ngmlr_b200_read_file_open(const char* path, const ngmlr_b200_read_file_options* opts, ngmlr_b200_read_file** out);
+void ngmlr_b200_read_file_close(ngmlr_b200_read_file* f);
+/* The next reads of the file -- at most max_reads (>= 1) and, after the first, no more than max_bases (<= 0: no
+ * limit) bases in all -- become ctx's resident read set exactly as ngmlr_b200_reads_upload(ctx, *n_reads, seqs, lens,
+ * read_part_length) with the strings ngmlr's ReadProvider makes: the name cut to 249 characters, bases upper-cased
+ * with everything but A / C / G / T as N, the quality string as it is ("*" for FASTA). reads (room for max_reads)
+ * receive name / seq / qual / length / empty with n_aln = 0, first_aln = 0, mapped = 0: ready for ngmlr_b200_sam_format once
+ * ngmlr_b200_map_short_reads has filled those three. An empty record gets length 0 and empty = 1 (ngmlr writes
+ * read_part_length + 16 N's and flags it Empty; no candidate and no SAM record can come of either). The strings
+ * are owned by f until its next load. A FASTQ record whose qualities are missing or of another length is dropped
+ * and ends the file, as ngmlr's "Length of read not equal length of quality values" error ends ngmlr: *n_dropped = 1
+ * and ngmlr_b200_reads_load_dropped names it. Returns the number of sub-reads (as reads_upload), or < 0;
+ * *n_reads == 0 at the end of the file. A record of 2^31 or more bases, a read error and a corrupt or truncated
+ * gzip stream are errors. */
+int ngmlr_b200_reads_load(ngmlr_b200_ctx* ctx, ngmlr_b200_read_file* f, int max_reads, int64_t max_bases,
+                          int read_part_length, ngmlr_b200_sam_read* reads, int* n_reads, int* n_dropped);
+/* Name of the read the last ngmlr_b200_reads_load dropped (cut as ngmlr cuts it), or NULL. */
+const char* ngmlr_b200_reads_load_dropped(const ngmlr_b200_read_file* f);
+/* Timings and sizes of the handle so far: bytes of stream read, records, milliseconds reading / inflating on the host,
+ * in the device parse, gathering + copying back, and the most device memory the handle held. Any pointer may be NULL. */
+int ngmlr_b200_read_file_stats(const ngmlr_b200_read_file* f, int64_t* stream_bytes, int64_t* records, float* read_ms,
+                               float* parse_ms, float* gather_ms, int64_t* device_bytes);
+
 #ifdef __cplusplus
 }
 #endif

@@ -69,6 +69,8 @@ C_API_SYMBOLS = (
     "ngmlr_b200_ngm_write_reference", "ngmlr_b200_ngm_read_reference", "ngmlr_b200_cs_encode_reference",
     "ngmlr_b200_cs_get_reference", "ngmlr_b200_dedupe_short_read_candidates", "ngmlr_b200_score_short_reads",
     "ngmlr_b200_map_short_reads", "ngmlr_b200_load_reference", "ngmlr_b200_reference_contigs",
+    "ngmlr_b200_read_file_open", "ngmlr_b200_read_file_close", "ngmlr_b200_reads_load", "ngmlr_b200_reads_load_dropped",
+    "ngmlr_b200_read_file_stats",
 )
 
 # flags of ngmlr_b200_load_reference (include/ngmlr_b200.h)
@@ -77,6 +79,12 @@ LOAD_REFERENCE_READ, LOAD_REFERENCE_WRITTEN, LOAD_INDEX_READ, LOAD_INDEX_WRITTEN
 
 class ReferenceOptions(C.Structure):
     _fields_ = [(k, C.c_int32) for k in ("k", "kmer_skip", "bin_shift", "max_prefix_freq", "skip_write", "rebuild")]
+
+
+class ReadFileOptions(C.Structure):
+    _fields_ = [("chunk_bytes", C.c_int64)]
+
+
 PLUGIN_SYMBOLS = ("CreateAlignment", "DeleteAlignment", "SetAlignmentScoring")
 
 _lib = None
@@ -177,6 +185,16 @@ def load():
     lib.ngmlr_b200_load_reference_ms.argtypes = [vp, C.POINTER(C.c_float)]
     lib.ngmlr_b200_debug_read_fasta.argtypes = [C.c_char_p, C.c_uint64, i64p, u64p, u64p, u64p, i64p, u64p, C.c_char_p,
                                                 C.c_char_p, C.c_char_p, C.c_int]
+    # the records' type is samtext.SamRead (an untyped pointer here, as for map_short_reads)
+    lib.ngmlr_b200_read_file_open.argtypes = [C.c_char_p, C.POINTER(ReadFileOptions), C.POINTER(vp)]
+    lib.ngmlr_b200_read_file_close.argtypes = [vp]
+    lib.ngmlr_b200_read_file_close.restype = None
+    lib.ngmlr_b200_reads_load.argtypes = [vp, vp, C.c_int, C.c_int64, C.c_int, vp, i32p, i32p]
+    lib.ngmlr_b200_reads_load_dropped.argtypes = [vp]
+    lib.ngmlr_b200_reads_load_dropped.restype = C.c_char_p
+    f32p = C.POINTER(C.c_float)
+    lib.ngmlr_b200_read_file_stats.argtypes = [vp, i64p, i64p, f32p, f32p, f32p, i64p]
+    lib.ngmlr_b200_debug_resident_reads.argtypes = [vp, i32p, i32p, i64p, vp, vp, vp, vp, vp]
     lib.ngmlr_b200_sw_last_kernel_ms.argtypes = [vp]
     lib.ngmlr_b200_sw_last_kernel_ms.restype = C.c_float
     lib.ngmlr_b200_plugin_context.argtypes = [vp]

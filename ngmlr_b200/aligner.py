@@ -210,6 +210,15 @@ class IntervalBatch:
                 a += 1
 
 
+@dataclass
+class ReadBatch:
+    """One ngmlr_b200_reads_load call: samtext.Read records, the number of sub-reads of the resident set, and the name
+    of a read ngmlr would have dropped (quality length differs from the sequence length; it ends the file)."""
+    reads: list
+    n_sub: int
+    dropped: list
+
+
 class B200Aligner:
     def __init__(self, gpu_id=0, scoring=DEFAULT_SCORING, stream=None):
         self.lib = _lib.load()
@@ -476,6 +485,58 @@ class B200Aligner:
         self._cs_n = n_sub
         self._cs_reads = reads.n
         return n_sub
+
+    def load_reads(self, path, read_part_length=256, max_reads=100_000, max_bases=0, chunk_bytes=0):
+        """Reads a FASTA / FASTQ file (plain or gzip) as ngmlr's ReadProvider reads its query file, parsed on the device
+        (ngmlr_b200_reads_load). Yields one ReadBatch per call: its reads -- at most max_reads, and after the first no
+        more than max_bases bases (0: no limit) -- are this context's resident read set while the batch is current,
+        exactly as reads_upload would make them (cs_run / map_short_reads follow), and its `reads` are samtext.Read
+        records (name, normalised bases, quality) for sam_format. A read ngmlr would drop for a quality string of
+        another length ends the file; its name is in the last batch's `dropped`."""
+        from .samtext import Read, SamRead
+        f = C.c_void_p()
+        opts = _lib.ReadFileOptions(int(chunk_bytes))
+        if self.lib.ngmlr_b200_read_file_open(os.fsencode(path), C.byref(opts), C.byref(f)) != 0:
+            raise RuntimeError(self.lib.ngmlr_b200_last_error(None).decode())
+        try:
+            recs = (SamRead * max(int(max_reads), 1))()
+            n, nd = C.c_int32(0), C.c_int32(0)
+            while True:
+                n_sub = self._check(self.lib.ngmlr_b200_reads_load(self.h, f, int(max_reads), int(max_bases),
+                                                                   int(read_part_length), recs, C.byref(n),
+                                                                   C.byref(nd)))
+                self._cs_n = n_sub
+                self._cs_reads = n.value
+                reads = []
+                base, size = C.addressof(recs), C.sizeof(SamRead)
+                ptr = lambda i, fld: C.c_void_p.from_address(base + i * size + getattr(SamRead, fld).offset).value
+                for i in range(n.value):
+                    r = recs[i]
+                    seq = C.string_at(ptr(i, "seq"), r.length)
+                    qual = C.string_at(ptr(i, "qual"), 2)  # "*" (FASTA, or no qualities) is NUL terminated
+                    qual = b"*" if qual == b"*\0" else C.string_at(ptr(i, "qual"), r.length)
+                    reads.append(Read(C.string_at(ptr(i, "name")), seq, qual, empty=bool(r.empty)))
+                dropped = [self.lib.ngmlr_b200_reads_load_dropped(f)] if nd.value else []
+                if reads or dropped:
+                    yield ReadBatch(reads, n_sub, dropped)
+                if n.value == 0:
+                    break
+        finally:
+            self.lib.ngmlr_b200_read_file_close(f)
+
+    def resident_reads(self):
+        """Test aid: the resident read set as the device holds it -- (read offsets, read lengths, sub-read offsets,
+        sub-read lengths, arena bytes)."""
+        n, m, nb = C.c_int32(0), C.c_int32(0), C.c_int64(0)
+        self._check(self.lib.ngmlr_b200_debug_resident_reads(self.h, C.byref(n), C.byref(m), C.byref(nb), *[None] * 5))
+        off = np.zeros(n.value + 1, dtype=np.uint64)
+        ln = np.zeros(max(n.value, 1), dtype=np.int32)
+        soff = np.zeros(max(m.value, 1), dtype=np.uint64)
+        slen = np.zeros(max(m.value, 1), dtype=np.int32)
+        arena = np.zeros(max(nb.value, 1), dtype=np.uint8)
+        self._check(self.lib.ngmlr_b200_debug_resident_reads(self.h, None, None, None, off.ctypes.data, ln.ctypes.data,
+                                                             soff.ctypes.data, slen.ctypes.data, arena.ctypes.data))
+        return off if n.value else off[:1], ln[:n.value], soff[:m.value], slen[:m.value], arena[:nb.value]
 
     def reads_h2d_bytes(self):
         return int(self.lib.ngmlr_b200_reads_h2d_bytes(self.h))

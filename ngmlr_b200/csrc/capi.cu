@@ -28,6 +28,8 @@ std::string g_create_error;
 
 }  // namespace
 
+void nb::set_error_without_context(const std::string& msg) { g_create_error = msg; }
+
 namespace nb {
 
 // When may a batch take the scalar-rule kernel? The as-coded SSE fill (raw indelRun in the run tests) and the

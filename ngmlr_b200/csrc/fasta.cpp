@@ -31,16 +31,14 @@ constexpr size_t CHUNK = 16384;
 bool is_space(int c) { return c == ' ' || c == '\t' || c == '\n' || c == '\v' || c == '\f' || c == '\r'; }
 
 struct Input {
-  gzFile f = nullptr;
+  StreamFile* f = nullptr;
   unsigned char buf[CHUNK];
   size_t b = 0, e = 0;
   bool eof = false, bad = false;
-  ~Input() {
-    if (f) gzclose(f);
-  }
+  ~Input() { close_stream(f); }
   // refill: false when nothing more can be read
   bool fill() {
-    const int n = gzread(f, buf, CHUNK);
+    const int64_t n = read_stream(f, buf, CHUNK);
     if (n < 0) {
       bad = true;
       eof = true;
@@ -81,6 +79,43 @@ struct Input {
 
 }  // namespace
 
+struct StreamFile {
+  gzFile gz = nullptr;
+};
+
+StreamFile* open_stream(const char* path) {
+  gzFile gz = gzopen(path, "rb");
+  if (!gz) return nullptr;
+  gzbuffer(gz, 1 << 20);
+  StreamFile* f = new StreamFile;
+  f->gz = gz;
+  return f;
+}
+
+void close_stream(StreamFile* f) {
+  if (!f) return;
+  gzclose(f->gz);
+  delete f;
+}
+
+int64_t read_stream(StreamFile* f, void* buf, size_t n) {
+  size_t got = 0;
+  while (got < n) {
+    const unsigned want = (unsigned)std::min<size_t>(n - got, 1u << 30);
+    const int r = gzread(f->gz, static_cast<char*>(buf) + got, want);
+    if (r < 0) return -1;
+    got += (size_t)r;
+    if ((unsigned)r < want) break;
+  }
+  return (int64_t)got;
+}
+
+bool stream_truncated(StreamFile* f) {
+  int errnum = Z_OK;
+  gzerror(f->gz, &errnum);
+  return errnum != Z_OK;
+}
+
 void FastaText::release_text() {
   if (text) {
     if (pinned)
@@ -120,9 +155,8 @@ int read_fasta(const char* path, bool pinned, uint64_t max_concat_len, FastaText
   const long file_size = ftell(probe);
   fclose(probe);
   Input in;
-  in.f = gzopen(path, "rb");
+  in.f = open_stream(path);
   if (!in.f) return fail(-2, "cannot open %s", path);
-  gzbuffer(in.f, 1 << 20);
   out.pinned = pinned;
   bool oom = false;
   // room for n more bytes of text: the file size for plain files, grown by doubling for compressed ones

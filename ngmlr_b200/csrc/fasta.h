@@ -34,6 +34,16 @@ struct FastaText {
 // Returns 0, or < 0 with a message in err.
 int read_fasta(const char* path, bool pinned, uint64_t max_concat_len, FastaText& out, std::string& err);
 
+// The byte stream ngmlr's readers see through gzopen / gzread: a plain file as it is, a gzip file inflated.
+// open_stream returns NULL when the file cannot be opened. read_stream reads up to n bytes (fewer only at the end of
+// the stream) and returns the count, or -1 on a read error or a corrupt gzip stream. stream_truncated tells, once
+// read_stream has returned 0, whether the gzip stream stopped before its end (zlib's gzread reports that as an end).
+struct StreamFile;
+StreamFile* open_stream(const char* path);
+void close_stream(StreamFile* f);
+int64_t read_stream(StreamFile* f, void* buf, size_t n);
+bool stream_truncated(StreamFile* f);
+
 // Length of the concatenated genome _SequenceProvider::Init builds from records of these lengths (1000-N spacers
 // before, between and after the contigs of more than 10 bases, each contig starting on a byte boundary).
 uint64_t concat_len_of(const std::vector<uint64_t>& lens);

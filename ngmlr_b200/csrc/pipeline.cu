@@ -190,6 +190,52 @@ int prepare_intervals(ngmlr_b200_ctx* ctx, CsState* cs, int n, const ngmlr_b200_
 
 }  // namespace
 
+namespace nb {
+
+int read_set_layout(ngmlr_b200_ctx* ctx, const char* who, int n_reads, const int32_t* lens, int read_part_length,
+                    std::vector<uint64_t>& sub_start, ReadSetShape& shape) {
+  ctx->read_off.resize((size_t)n_reads + 1);
+  ctx->read_len.assign(lens, lens + n_reads);
+  sub_start.resize((size_t)n_reads + 1);
+  shape = ReadSetShape();
+  for (int i = 0; i < n_reads; ++i) {
+    if (lens[i] < 0) return ctx->fail("%s: negative length at %d", who, i);
+    ctx->read_off[i] = shape.bytes;
+    sub_start[i] = shape.n_sub;
+    shape.bytes += align_up((size_t)lens[i] + 1, 16);
+    const int parts = lens[i] / read_part_length;
+    shape.n_sub += parts > 0 ? (size_t)parts : 1;  // a read shorter than one part is its own sub-read (:76-104)
+    shape.max_sub = std::max(shape.max_sub, parts > 0 ? read_part_length : lens[i]);
+  }
+  ctx->read_off[n_reads] = shape.bytes;
+  sub_start[n_reads] = shape.n_sub;
+  if (shape.n_sub > 0x7fffffffull) return ctx->fail("%s: too many sub-reads", who);
+  return 0;
+}
+
+int read_set_reserve(ngmlr_b200_ctx* ctx, CsState* cs, int n_reads, const ReadSetShape& shape) {
+  CU(ctx->d_reads.reserve(shape.bytes + 64));
+  CU(ctx->d_read_off.reserve((size_t)n_reads + 1));
+  CU(cs->d_off.reserve(shape.n_sub + 1));
+  CU(cs->d_len.reserve(shape.n_sub + 1));
+  return 0;
+}
+
+void read_set_install(ngmlr_b200_ctx* ctx, CsState* cs, int n_reads, const ReadSetShape& shape) {
+  ctx->n_reads = n_reads;
+  ctx->reads_bytes = shape.bytes;
+  // stage 0/2 now runs on the sub-reads of the resident set (ngmlr_b200_cs_run / cs_fetch)
+  cs->rn = (int)shape.n_sub;
+  cs->rmax = shape.max_sub;
+  cs->rbytes = shape.bytes;
+  cs->seq_base = ctx->d_reads.p;
+  cs->n_cand = 0;
+  cs->reads_searched = false;
+  ctx->reads_h2d_bytes = (int64_t)(shape.bytes + ((size_t)n_reads + 1) * 8 + shape.n_sub * 12);
+}
+
+}  // namespace nb
+
 extern "C" {
 
 int ngmlr_b200_reads_upload(ngmlr_b200_ctx* ctx, int n_reads, const char* const* seqs, const int32_t* lens,
@@ -200,20 +246,10 @@ int ngmlr_b200_reads_upload(ngmlr_b200_ctx* ctx, int n_reads, const char* const*
   CU(cudaSetDevice(ctx->device));
   cudaStream_t st = ctx->stream;
   CsState* cs = cs_state(ctx, true);
-  ctx->read_off.resize((size_t)n_reads + 1);
-  ctx->read_len.assign(lens, lens + n_reads);
-  size_t bytes = 0, n_sub = 0;
-  int max_sub = 0;  // the longest sub-read
-  for (int i = 0; i < n_reads; ++i) {
-    if (lens[i] < 0) return ctx->fail("reads_upload: negative length at %d", i);
-    ctx->read_off[i] = bytes;
-    bytes += align_up((size_t)lens[i] + 1, 16);
-    const int parts = lens[i] / read_part_length;
-    n_sub += parts > 0 ? (size_t)parts : 1;  // a read shorter than one part is its own sub-read (:76-104)
-    max_sub = std::max(max_sub, parts > 0 ? read_part_length : lens[i]);
-  }
-  ctx->read_off[n_reads] = bytes;
-  if (n_sub > 0x7fffffffull) return ctx->fail("reads_upload: too many sub-reads");
+  std::vector<uint64_t> sub_start;
+  ReadSetShape shape;
+  if (read_set_layout(ctx, "reads_upload", n_reads, lens, read_part_length, sub_start, shape)) return -1;
+  const size_t bytes = shape.bytes, n_sub = shape.n_sub;
   // one pinned staging block: read bytes | read offsets | sub-read offsets | sub-read lengths
   const size_t off_at = align_up(bytes + 16, 16), soff_at = off_at + ((size_t)n_reads + 1) * 8,
                slen_at = soff_at + (n_sub + 1) * 8, total = slen_at + (n_sub + 1) * 4;
@@ -240,10 +276,7 @@ int ngmlr_b200_reads_upload(ngmlr_b200_ctx* ctx, int n_reads, const char* const*
       }
     }
   }
-  CU(ctx->d_reads.reserve(bytes + 64));
-  CU(ctx->d_read_off.reserve((size_t)n_reads + 1));
-  CU(cs->d_off.reserve(n_sub + 1));
-  CU(cs->d_len.reserve(n_sub + 1));
+  if (read_set_reserve(ctx, cs, n_reads, shape)) return -1;
   CU(cudaMemcpyAsync(ctx->d_reads.p, h, bytes, cudaMemcpyHostToDevice, st));
   CU(cudaMemcpyAsync(ctx->d_read_off.p, h + off_at, ((size_t)n_reads + 1) * 8, cudaMemcpyHostToDevice, st));
   if (n_sub) {
@@ -251,16 +284,7 @@ int ngmlr_b200_reads_upload(ngmlr_b200_ctx* ctx, int n_reads, const char* const*
     CU(cudaMemcpyAsync(cs->d_len.p, slen, n_sub * 4, cudaMemcpyHostToDevice, st));
   }
   CU(nb_stream_sync(ctx, st));
-  ctx->n_reads = n_reads;
-  ctx->reads_bytes = bytes;
-  // stage 0/2 now runs on the sub-reads of the resident set (ngmlr_b200_cs_run / cs_fetch)
-  cs->rn = (int)n_sub;
-  cs->rmax = max_sub;
-  cs->rbytes = bytes;
-  cs->seq_base = ctx->d_reads.p;
-  cs->n_cand = 0;
-  cs->reads_searched = false;
-  ctx->reads_h2d_bytes = (int64_t)(bytes + ((size_t)n_reads + 1) * 8 + n_sub * 12);
+  read_set_install(ctx, cs, n_reads, shape);
   return (int)n_sub;
 }
 

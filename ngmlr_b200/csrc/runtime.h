@@ -442,6 +442,23 @@ struct CsState {
 
 CsState* cs_state(ngmlr_b200_ctx* ctx, bool create);
 
+// What ngmlr_b200_last_error(NULL) reports (calls that take no context: create, read_file_open).
+void set_error_without_context(const std::string& msg);
+
+// The resident read set of ngmlr_b200_reads_upload and ngmlr_b200_reads_load (pipeline.cu): reads back to back,
+// 16-byte aligned and NUL padded, and their sub-reads (ReadProvider::splitRead). read_set_layout fills
+// ctx->read_off / read_len and sub_start (the first sub-read of every read, n_reads + 1 entries) from the lengths;
+// read_set_reserve sizes the device arrays; read_set_install makes the set the one stage 0/2 and stage 4 run on,
+// once its bytes, offsets and sub-read table are on the device.
+struct ReadSetShape {
+  size_t bytes = 0, n_sub = 0;
+  int max_sub = 0;  // the longest sub-read
+};
+int read_set_layout(ngmlr_b200_ctx* ctx, const char* who, int n_reads, const int32_t* lens, int read_part_length,
+                    std::vector<uint64_t>& sub_start, ReadSetShape& shape);
+int read_set_reserve(ngmlr_b200_ctx* ctx, CsState* cs, int n_reads, const ReadSetShape& shape);
+void read_set_install(ngmlr_b200_ctx* ctx, CsState* cs, int n_reads, const ReadSetShape& shape);
+
 int convex_upload_spec(ngmlr_b200_ctx* ctx, const UploadSpec& spec);
 
 // Fill kernel choice (capi.cu): whether a batch under scoring `s` whose scores stay below `magnitude` needs the RAW
