@@ -392,8 +392,8 @@ int ngmlr_b200_ngm_read_reference(const char* path, uint32_t* n_refs, uint64_t* 
  * (src/SequenceProvider.cpp:246-424, src/PrefixTable.cpp:97-128), with the encoding and the k-mer index built on the
  * device. In ngmlr's order:
  *   - <fasta>-enc.2.ngm exists: it is read and installed (ngmlr_b200_ngm_read_reference -> cs_set_reference +
- *     set_ref_starts); an invalid one is an error, as in ngmlr. Otherwise the FASTA / FASTQ file (plain or gzip) is
- *     read as ngmlr's kseq_read loop reads it, encoded on the device (cs_encode_reference) and the file is written
+ *     set_ref_starts); an invalid one is an error, as in ngmlr. Otherwise the FASTA / FASTQ file (plain, gzip or BGZF;
+ *     BGZF inflated on the device, see ngmlr_b200_reads_load) is read as ngmlr's kseq_read loop reads it, encoded on the device (cs_encode_reference) and the file is written
  *     unless skip_write.
  *   - <fasta>-ht-<k>-<kmer_skip>.2.ngm exists and is a valid single-unit table for k / kmer_skip: it is read and
  *     installed (cs_set_index). Otherwise the index is built on the device (cs_build_index) and written unless
@@ -424,6 +424,12 @@ int ngmlr_b200_load_reference(ngmlr_b200_ctx* ctx, const char* fasta_path, const
  * of contigs, or < 0 when the context's reference did not come from load_reference. */
 int ngmlr_b200_reference_contigs(ngmlr_b200_ctx* ctx, const char** names, int32_t* name_lens, uint64_t* starts,
                                  uint64_t* lens);
+/* What reading the FASTA file of the context's last load_reference took from the file: bytes read from it, BGZF
+ * members inflated on the device, bytes inflated by the host continuation (see ngmlr_b200_read_file_inflate_stats)
+ * and device inflate milliseconds; all 0 when the caches were read, gzread counts only the bytes read. Any pointer
+ * may be NULL. Returns 0 or < 0. */
+int ngmlr_b200_load_reference_inflate_stats(ngmlr_b200_ctx* ctx, int64_t* compressed_bytes, int64_t* device_members,
+                                            int64_t* host_bytes, float* inflate_ms);
 
 /* ---- SAM text (SURVEY section 8(f)4) ----------------------------------------------------------
  * Replaces SAMWriter::DoWriteProlog / DoWriteRead -> DoWriteReadGeneric / DoWriteUnmappedRead
@@ -539,13 +545,17 @@ int ngmlr_b200_map_short_reads(ngmlr_b200_ctx* ctx, int read_part_length, float 
                                int64_t* first_aln, int32_t* mapped, const ngmlr_b200_sam_aln** alns,
                                int64_t* n_alns_total);
 
-/* ---- reads from a FASTA / FASTQ file (plain or gzip): ReadProvider::NextRead -> FastXParser -> kseq_read ->
+/* ---- reads from a FASTA / FASTQ file (plain, gzip or BGZF): ReadProvider::NextRead -> FastXParser -> kseq_read ->
  * IParser::copyToRead (src/ReadProvider.cpp:136-187, src/IParser.h:51-117), parsed on the device ------------------
- * The file is read in chunks of chunk_bytes (0: 256 MiB) into page-locked memory (gzip inflated by zlib on the calling
- * thread); a chunk too small for one record grows. Each chunk goes to the device once: its line table, the record
- * structure (kseq's rules, multi-line FASTQ and quality lines starting with '@' / '>' included) and the normalised
- * bases are computed there. Device memory of a handle stays below 9 x chunk_bytes. No reference counterpart for
- * the handle itself. */
+ * The file is read in chunks of chunk_bytes (0: 256 MiB) into page-locked memory; a chunk too small for one record
+ * grows. Compressed input: a BGZF file (first member header 1f 8b 08, FLG 0x04 with a BC extra subfield, as bgzip /
+ * htslib write it) is inflated on the context's device, one warp per member, from the first reads_load on; from the
+ * first member the device cannot vouch for (anything zlib would refuse or read differently), and for every other gzip
+ * file, zlib inflates on the calling thread exactly as gzread does. Each chunk goes to the device once: its line
+ * table, the record structure (kseq's rules, multi-line FASTQ and quality lines starting with '@' / '>' included) and
+ * the normalised bases are computed there. Device memory of a handle stays below 9 x chunk_bytes, and for BGZF input
+ * (which adds the compressed staging and the inflated output of a round) below 11 x max(chunk_bytes, 1 MiB). No
+ * reference counterpart for the handle itself. */
 typedef struct ngmlr_b200_read_file ngmlr_b200_read_file;
 typedef struct {
   int64_t chunk_bytes; /* page-locked staging per chunk; 0 = 256 MiB; grows for a larger record */
@@ -573,6 +583,11 @@ const char* ngmlr_b200_reads_load_dropped(const ngmlr_b200_read_file* f);
  * in the device parse, gathering + copying back, and the most device memory the handle held. Any pointer may be NULL. */
 int ngmlr_b200_read_file_stats(const ngmlr_b200_read_file* f, int64_t* stream_bytes, int64_t* records, float* read_ms,
                                float* parse_ms, float* gather_ms, int64_t* device_bytes);
+/* How the handle's file was inflated so far: bytes read from the file, BGZF members inflated on the device, bytes
+ * inflated by the host continuation (zlib, from the first member the device could not vouch for), and milliseconds
+ * of the device inflate kernel (CUDA events). Any pointer may be NULL. */
+int ngmlr_b200_read_file_inflate_stats(const ngmlr_b200_read_file* f, int64_t* compressed_bytes,
+                                       int64_t* device_members, int64_t* host_bytes, float* inflate_ms);
 
 #ifdef __cplusplus
 }

@@ -36,6 +36,12 @@ class LoadedReference:
     index_read: bool
     index_written: bool
     ms: dict
+    # the FASTA file's inflate (0 when the caches were read): bytes read from the file, BGZF members inflated on the
+    # device, bytes inflated by the host continuation, device inflate milliseconds
+    compressed_bytes: int = 0
+    device_members: int = 0
+    host_bytes: int = 0
+    inflate_ms: float = 0.0
 
     def sam_ref_names(self):
         """The reference list SAM records index (ids count both strands): every name twice."""
@@ -213,10 +219,16 @@ class IntervalBatch:
 @dataclass
 class ReadBatch:
     """One ngmlr_b200_reads_load call: samtext.Read records, the number of sub-reads of the resident set, and the name
-    of a read ngmlr would have dropped (quality length differs from the sequence length; it ends the file)."""
+    of a read ngmlr would have dropped (quality length differs from the sequence length; it ends the file). The inflate
+    counters are the handle's so far: bytes read from the file, BGZF members inflated on the device, bytes inflated by
+    the host continuation, device inflate milliseconds."""
     reads: list
     n_sub: int
     dropped: list
+    compressed_bytes: int = 0
+    device_members: int = 0
+    host_bytes: int = 0
+    inflate_ms: float = 0.0
 
 
 class B200Aligner:
@@ -363,7 +375,7 @@ class B200Aligner:
 
     def load_reference(self, path, k=13, kmer_skip=2, bin_shift=4, skip_write=False, rebuild=False, max_prefix_freq=1000):
         """ngmlr's start-up (ngmlr_b200_load_reference): the reference and its k-mer index from <path>-enc.2.ngm and
-        <path>-ht-<k>-<kmer_skip>.2.ngm where they exist, else from the FASTA / FASTQ file (plain or gzip) with the
+        <path>-ht-<k>-<kmer_skip>.2.ngm where they exist, else from the FASTA / FASTQ file (plain, gzip or BGZF) with the
         encoding and the index built on the device and both caches written next to it (unless skip_write). Installs
         the reference, refStartPos and the index in this context. Returns a LoadedReference: the contig table (names
         cut to 100 characters, SeqStart, SeqLen), which cache files were read / written, and the phase times."""
@@ -381,11 +393,15 @@ class B200Aligner:
         ms = (C.c_float * 6)()
         self._check(self.lib.ngmlr_b200_load_reference_ms(self.h, ms))
         f = fl.value
+        cb, dm, hb, ims = C.c_int64(0), C.c_int64(0), C.c_int64(0), C.c_float(0)
+        self._check(self.lib.ngmlr_b200_load_reference_inflate_stats(self.h, C.byref(cb), C.byref(dm), C.byref(hb),
+                                                                      C.byref(ims)))
         return LoadedReference([names[i][:int(nlen[i])] for i in range(n.value)], [int(x) for x in starts],
                                [int(x) for x in lens], int(cl.value),
                                bool(f & _lib.LOAD_REFERENCE_READ), bool(f & _lib.LOAD_REFERENCE_WRITTEN),
                                bool(f & _lib.LOAD_INDEX_READ), bool(f & _lib.LOAD_INDEX_WRITTEN),
-                               dict(zip(LoadedReference.PHASES, [float(x) for x in ms])))
+                               dict(zip(LoadedReference.PHASES, [float(x) for x in ms])),
+                               cb.value, dm.value, hb.value, float(ims.value))
 
     def set_reference(self, ref):
         """ref: ngmlr_b200.refindex.EncodedReference (the reference's 4-bit `binRef`)."""
@@ -487,7 +503,7 @@ class B200Aligner:
         return n_sub
 
     def load_reads(self, path, read_part_length=256, max_reads=100_000, max_bases=0, chunk_bytes=0):
-        """Reads a FASTA / FASTQ file (plain or gzip) as ngmlr's ReadProvider reads its query file, parsed on the device
+        """Reads a FASTA / FASTQ file (plain, gzip or BGZF) as ngmlr's ReadProvider reads its query file, parsed on the device
         (ngmlr_b200_reads_load). Yields one ReadBatch per call: its reads -- at most max_reads, and after the first no
         more than max_bases bases (0: no limit) -- are this context's resident read set while the batch is current,
         exactly as reads_upload would make them (cs_run / map_short_reads follow), and its `reads` are samtext.Read
@@ -518,7 +534,9 @@ class B200Aligner:
                     reads.append(Read(C.string_at(ptr(i, "name")), seq, qual, empty=bool(r.empty)))
                 dropped = [self.lib.ngmlr_b200_reads_load_dropped(f)] if nd.value else []
                 if reads or dropped:
-                    yield ReadBatch(reads, n_sub, dropped)
+                    cb, dm, hb, ims = C.c_int64(0), C.c_int64(0), C.c_int64(0), C.c_float(0)
+                    self.lib.ngmlr_b200_read_file_inflate_stats(f, C.byref(cb), C.byref(dm), C.byref(hb), C.byref(ims))
+                    yield ReadBatch(reads, n_sub, dropped, cb.value, dm.value, hb.value, float(ims.value))
                 if n.value == 0:
                     break
         finally:

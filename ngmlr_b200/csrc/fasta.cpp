@@ -15,12 +15,18 @@
 #include "fasta.h"
 
 #include <cuda_runtime.h>
+#include <fcntl.h>
+#include <sys/stat.h>
+#include <unistd.h>
 #include <zlib.h>
 
 #include <algorithm>
+#include <cerrno>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <functional>
+#include <memory>
 
 namespace nb {
 
@@ -77,28 +83,532 @@ struct Input {
   }
 };
 
+constexpr size_t GZ_BUFFER = 1 << 20;           // gzbuffer() of open_stream: gzread reads 1 MiB, inflates 2 MiB
+constexpr int64_t READ_BLOCK = 4 << 20;         // read() size of the BGZF walker
+constexpr int64_t MIN_COMP_ROUND = 1 << 20;     // compressed bytes a round may always take
+constexpr int64_t MEMBERS_PER_BYTE = 4096;      // a round holds at most one member per 4 KiB of that budget (>= 64)
+
+// Host memory that grows keeping its first `keep` bytes; page-locked once the stream is bound to a device.
+struct HostBuf {
+  uint8_t* p = nullptr;
+  size_t cap = 0;
+  bool pinned = false;
+  bool reserve(size_t n, size_t keep) {
+    if (n <= cap) return true;
+    const size_t want = std::max(n, cap + cap / 2);
+    uint8_t* q = nullptr;
+    if (pinned) {
+      if (cudaMallocHost(&q, want) != cudaSuccess) return false;
+    } else if (!(q = static_cast<uint8_t*>(malloc(want)))) {
+      return false;
+    }
+    if (keep) memcpy(q, p, keep);
+    release();
+    p = q;
+    cap = want;
+    return true;
+  }
+  bool set_pinned(size_t keep) {
+    if (pinned) return true;
+    HostBuf b;
+    b.pinned = true;
+    if (!b.reserve(std::max<size_t>(keep, 1), 0)) return false;
+    if (keep) memcpy(b.p, p, keep);
+    std::swap(p, b.p);
+    std::swap(cap, b.cap);
+    std::swap(pinned, b.pinned);
+    return true;
+  }
+  void release() {
+    if (p) {
+      if (pinned) cudaFreeHost(p);
+      else free(p);
+    }
+    p = nullptr;
+    cap = 0;
+  }
+  ~HostBuf() { release(); }
+};
+
+// Device memory sized to the largest round so far (64 KiB granules, no slack: the read loader's bound counts it).
+template <typename T>
+struct DevMem {
+  T* p = nullptr;
+  size_t cap = 0;
+  cudaError_t reserve(size_t n) {
+    if (n <= cap) return cudaSuccess;
+    const size_t want = (n * sizeof(T) + 65535) / 65536 * 65536 / sizeof(T);
+    if (p) cudaFree(p);
+    p = nullptr;
+    cap = 0;
+    const cudaError_t e = cudaMalloc(&p, want * sizeof(T));
+    if (e == cudaSuccess) cap = want;
+    return e;
+  }
+  size_t bytes() const { return cap * sizeof(T); }
+  ~DevMem() {
+    if (p) cudaFree(p);
+  }
+};
+
+// gzread over a byte source, from the start of a file (fresh) or from the header of a member that follows another
+// one: zlib's gz_read / gz_fetch / gz_decomp / gz_look / gz_avail with the buffer sizes open_stream gives gzread.
+// gzread inflates a member into its 2 MiB buffer as soon as one byte of it is wanted, and reports an error in the call
+// that meets it; so this gives the same bytes from the same calls, the same -1 and the same truncation flag.
+class GzTail {
+ public:
+  using Source = std::function<int64_t(uint8_t*, size_t)>;  // up to n bytes; 0 at the end; < 0 on a read error
+  GzTail(Source src, bool fresh) : src_(std::move(src)), direct_(fresh), in_(GZ_BUFFER), out_(2 * GZ_BUFFER) {
+    memset(&strm_, 0, sizeof strm_);
+    ok_ = inflateInit2(&strm_, 15 + 16) == Z_OK;
+    if (!ok_) err_ = Z_MEM_ERROR;
+  }
+  ~GzTail() {
+    if (ok_) inflateEnd(&strm_);
+  }
+  int64_t read(uint8_t* buf, size_t len) {
+    if (err_ != Z_OK && err_ != Z_BUF_ERROR) return -1;
+    if (len == 0) return 0;
+    const size_t r = gz_read(buf, len);
+    if (r == 0 && err_ != Z_OK && err_ != Z_BUF_ERROR) return -1;
+    return (int64_t)r;
+  }
+  bool truncated() const { return err_ != Z_OK; }
+
+ private:
+  enum { LOOK, COPY, GZIP };
+  int load(uint8_t* buf, size_t n, size_t* have) {
+    *have = 0;
+    int64_t r = 0;
+    do {
+      r = src_(buf + *have, n - *have);
+      if (r <= 0) break;
+      *have += (size_t)r;
+    } while (*have < n);
+    if (r < 0) {
+      err_ = Z_ERRNO;
+      return -1;
+    }
+    if (r == 0) eof_ = true;
+    return 0;
+  }
+  int avail() {
+    if (err_ != Z_OK && err_ != Z_BUF_ERROR) return -1;
+    if (!eof_) {
+      if (strm_.avail_in) memmove(in_.data(), strm_.next_in, strm_.avail_in);
+      size_t got = 0;
+      if (load(in_.data() + strm_.avail_in, GZ_BUFFER - strm_.avail_in, &got) == -1) return -1;
+      strm_.avail_in += (unsigned)got;
+      strm_.next_in = in_.data();
+    }
+    return 0;
+  }
+  int look() {
+    if (strm_.avail_in < 2) {
+      if (avail() == -1) return -1;
+      if (strm_.avail_in == 0) return 0;
+    }
+    if (strm_.avail_in > 1 && strm_.next_in[0] == 31 && strm_.next_in[1] == 139) {
+      inflateReset(&strm_);
+      how_ = GZIP;
+      direct_ = false;
+      return 0;
+    }
+    if (!direct_) {  // after a gzip member: trailing garbage, ignored
+      strm_.avail_in = 0;
+      eof_ = true;
+      x_have_ = 0;
+      return 0;
+    }
+    x_next_ = out_.data();
+    memcpy(x_next_, strm_.next_in, strm_.avail_in);
+    x_have_ = strm_.avail_in;
+    strm_.avail_in = 0;
+    how_ = COPY;
+    return 0;
+  }
+  int decomp() {
+    int ret = Z_OK;
+    const unsigned had = strm_.avail_out;
+    do {
+      if (strm_.avail_in == 0 && avail() == -1) return -1;
+      if (strm_.avail_in == 0) {
+        err_ = Z_BUF_ERROR;  // "unexpected end of file"
+        break;
+      }
+      ret = inflate(&strm_, Z_NO_FLUSH);
+      if (ret == Z_STREAM_ERROR || ret == Z_NEED_DICT || ret == Z_MEM_ERROR || ret == Z_DATA_ERROR) {
+        err_ = ret == Z_NEED_DICT ? Z_STREAM_ERROR : ret;
+        return -1;
+      }
+    } while (strm_.avail_out && ret != Z_STREAM_END);
+    x_have_ = had - strm_.avail_out;
+    x_next_ = strm_.next_out - x_have_;
+    if (ret == Z_STREAM_END) how_ = LOOK;
+    return 0;
+  }
+  int fetch() {
+    do {
+      switch (how_) {
+        case LOOK:
+          if (look() == -1) return -1;
+          if (how_ == LOOK) return 0;
+          break;
+        case COPY: {
+          size_t h = 0;
+          if (load(out_.data(), out_.size(), &h) == -1) return -1;
+          x_have_ = h;
+          x_next_ = out_.data();
+          return 0;
+        }
+        case GZIP:
+          strm_.avail_out = (unsigned)out_.size();
+          strm_.next_out = out_.data();
+          if (decomp() == -1) return -1;
+      }
+    } while (x_have_ == 0 && (!eof_ || strm_.avail_in));
+    return 0;
+  }
+  size_t gz_read(uint8_t* buf, size_t len) {
+    size_t got = 0;
+    do {
+      size_t n = len;
+      if (x_have_) {
+        n = std::min(x_have_, len);
+        memcpy(buf, x_next_, n);
+        x_next_ += n;
+        x_have_ -= n;
+      } else if (eof_ && strm_.avail_in == 0) {
+        break;
+      } else if (how_ == LOOK || n < out_.size()) {
+        if (fetch() == -1) return 0;
+        continue;
+      } else if (how_ == COPY) {
+        if (load(buf, n, &n) == -1) return 0;
+      } else {
+        strm_.avail_out = (unsigned)n;
+        strm_.next_out = buf;
+        if (decomp() == -1) return 0;
+        n = x_have_;
+        x_have_ = 0;
+      }
+      len -= n;
+      buf += n;
+      got += n;
+    } while (len);
+    return got;
+  }
+
+  Source src_;
+  bool direct_, ok_ = false, eof_ = false;
+  int how_ = LOOK, err_ = Z_OK;
+  z_stream strm_;
+  std::vector<uint8_t> in_, out_;
+  uint8_t* x_next_ = nullptr;
+  size_t x_have_ = 0;
+};
+
+// One BGZF member as the walker sees it: file offset, header and total length (BSIZE + 1), trailer, output offset.
+struct Member {
+  int64_t c = 0, out = 0;
+  uint32_t hlen = 0, total = 0, crc = 0, isize = 0;
+};
+
+uint32_t le32(const uint8_t* p) { return p[0] | p[1] << 8 | p[2] << 16 | (uint32_t)p[3] << 24; }
+
 }  // namespace
 
 struct StreamFile {
   gzFile gz = nullptr;
+  // the BGZF walker (fd >= 0): the file read sequentially into stage = file bytes [stage_off, stage_off + stage_len)
+  int fd = -1;
+  HostBuf stage, out;
+  int64_t stage_off = 0, stage_len = 0;
+  bool file_eof = false;
+  int64_t next_c = 0;                 // file offset of the next member to walk
+  int64_t hold_b = 0, hold_e = 0;     // inflated bytes out[hold_b, hold_e) not yet returned
+  int64_t fallback_c = -1;            // where the host continuation starts once the held bytes are returned
+  bool ended = false;                 // the file ends after the held bytes
+  std::unique_ptr<GzTail> tail;
+  int64_t tail_pos = 0;               // file offset the continuation reads next
+  bool tail_fresh = false;            // the continuation starts at the file's first byte (a pipe that is not BGZF)
+  z_stream raw;
+  bool raw_init = false;
+  // the device binding
+  int device = -1;
+  cudaStream_t st = nullptr;
+  int64_t min_round = 0;
+  DevMem<uint8_t> d_comp, d_out;
+  DevMem<InflateMember> d_mem;
+  DevMem<int32_t> d_status;
+  std::vector<InflateMember> mem;
+  std::vector<int32_t> status;
+  cudaEvent_t ev[2] = {nullptr, nullptr};
+  StreamCounters cnt;
+  std::string error;
+  ~StreamFile() {
+    if (gz) gzclose(gz);
+    if (fd >= 0) close(fd);
+    if (raw_init) inflateEnd(&raw);
+    for (cudaEvent_t e : ev)
+      if (e) cudaEventDestroy(e);
+  }
 };
 
-StreamFile* open_stream(const char* path) {
+namespace {
+
+// File bytes up to `end` in the stage: 1, or 0 when the file ends first, or -1 on a read error / no memory.
+int stage_cover(StreamFile* f, int64_t end) {
+  while (f->stage_off + f->stage_len < end && !f->file_eof) {
+    const int64_t want = std::max<int64_t>(end - (f->stage_off + f->stage_len), READ_BLOCK);
+    if (!f->stage.reserve((size_t)(f->stage_len + want), (size_t)f->stage_len)) {
+      f->error = "out of host memory for the BGZF staging buffer";
+      return -1;
+    }
+    const ssize_t r = read(f->fd, f->stage.p + f->stage_len, (size_t)want);
+    if (r < 0) {
+      if (errno == EINTR) continue;
+      return -1;
+    }
+    if (r == 0) f->file_eof = true;
+    f->stage_len += r;
+    f->cnt.compressed_bytes += r;
+  }
+  return f->stage_off + f->stage_len >= end ? 1 : 0;
+}
+
+// The member at file offset c: 1 = a BGZF member whose bytes are staged, ISIZE <= 65536; 2 = the file ends at c;
+// 0 = anything else (another header, trailing bytes, a member running past the end of the file); -1 = read error.
+int walk_member(StreamFile* f, int64_t c, Member& m) {
+  int r = stage_cover(f, c + 18);
+  if (r < 0) return -1;
+  const int64_t avail = f->stage_off + f->stage_len - c;
+  if (avail == 0) return 2;
+  if (avail < 18) return 0;
+  const uint8_t* p = f->stage.p + (c - f->stage_off);
+  if (p[0] != 0x1f || p[1] != 0x8b || p[2] != 8 || p[3] != 4) return 0;
+  const uint32_t xlen = p[10] | p[11] << 8;
+  if ((r = stage_cover(f, c + 12 + xlen)) <= 0) return r;
+  p = f->stage.p + (c - f->stage_off);
+  int64_t total = -1;
+  for (uint32_t q = 0; q + 4 <= xlen;) {
+    const uint8_t* s = p + 12 + q;
+    const uint32_t slen = s[2] | s[3] << 8;
+    if (s[0] == 'B' && s[1] == 'C' && slen == 2 && q + 6 <= xlen) {
+      total = (s[4] | s[5] << 8) + 1;
+      break;
+    }
+    q += 4 + slen;
+  }
+  if (total < 12 + (int64_t)xlen + 8) return 0;
+  if ((r = stage_cover(f, c + total)) <= 0) return r;
+  p = f->stage.p + (c - f->stage_off);
+  m.c = c;
+  m.hlen = 12 + xlen;
+  m.total = (uint32_t)total;
+  m.crc = le32(p + total - 8);
+  m.isize = le32(p + total - 4);
+  return m.isize <= 65536 ? 1 : 0;
+}
+
+// How many of the round's leading members inflated to what zlib gives (their output is in f->out at m.out).
+int inflate_host(StreamFile* f, const std::vector<Member>& ms) {
+  if (!f->raw_init) {
+    memset(&f->raw, 0, sizeof f->raw);
+    if (inflateInit2(&f->raw, -15) != Z_OK) return 0;
+    f->raw_init = true;
+  }
+  int ok = 0;
+  for (const Member& m : ms) {
+    inflateReset(&f->raw);
+    f->raw.next_in = f->stage.p + (m.c - f->stage_off) + m.hlen;
+    f->raw.avail_in = m.total - m.hlen - 8;
+    f->raw.next_out = f->out.p + m.out;
+    f->raw.avail_out = m.isize;
+    const int ret = inflate(&f->raw, Z_FINISH);
+    if (ret != Z_STREAM_END || f->raw.avail_in || f->raw.avail_out ||
+        crc32(0, f->out.p + m.out, m.isize) != m.crc)
+      break;
+    ++ok;
+  }
+  return ok;
+}
+
+#define SCU(call)                                                                                   \
+  do {                                                                                              \
+    const cudaError_t e__ = (call);                                                                 \
+    if (e__ != cudaSuccess) {                                                                       \
+      f->error = std::string("BGZF inflate: ") + #call + " failed: " + cudaGetErrorString(e__);    \
+      return -1;                                                                                    \
+    }                                                                                               \
+  } while (0)
+
+// The same on the bound device: one warp per member (inflate.cu). Returns -1 on a CUDA error.
+int inflate_device(StreamFile* f, const std::vector<Member>& ms, int64_t out_bytes) {
+  const int n = (int)ms.size();
+  const int64_t c0 = ms.front().c, c1 = ms.back().c + ms.back().total;
+  f->mem.resize(n);
+  f->status.assign(n, -1);
+  for (int i = 0; i < n; ++i) {
+    const Member& m = ms[i];
+    f->mem[i] = InflateMember{(uint64_t)(m.c - c0 + m.hlen), (uint64_t)m.out, m.total - m.hlen - 8, m.isize, m.crc, 0};
+  }
+  SCU(cudaSetDevice(f->device));
+  SCU(f->d_comp.reserve((size_t)(c1 - c0) + 64));
+  SCU(f->d_out.reserve((size_t)out_bytes + 1));
+  SCU(f->d_mem.reserve(n));
+  SCU(f->d_status.reserve(n));
+  SCU(cudaMemcpyAsync(f->d_comp.p, f->stage.p + (c0 - f->stage_off), (size_t)(c1 - c0), cudaMemcpyHostToDevice, f->st));
+  SCU(cudaMemcpyAsync(f->d_mem.p, f->mem.data(), n * sizeof(InflateMember), cudaMemcpyHostToDevice, f->st));
+  SCU(cudaEventRecord(f->ev[0], f->st));
+  SCU(launch_inflate(f->d_comp.p, f->d_mem.p, n, f->d_out.p, f->d_status.p, f->st));
+  SCU(cudaEventRecord(f->ev[1], f->st));
+  if (out_bytes) SCU(cudaMemcpyAsync(f->out.p, f->d_out.p, (size_t)out_bytes, cudaMemcpyDeviceToHost, f->st));
+  SCU(cudaMemcpyAsync(f->status.data(), f->d_status.p, n * sizeof(int32_t), cudaMemcpyDeviceToHost, f->st));
+  SCU(cudaStreamSynchronize(f->st));
+  float ms_ = 0;
+  SCU(cudaEventElapsedTime(&ms_, f->ev[0], f->ev[1]));
+  f->cnt.inflate_ms += ms_;
+  int ok = 0;
+  while (ok < n && f->status[ok] == 0) ++ok;
+  f->cnt.device_members += ok;
+  return ok;
+}
+
+// One round from next_c: the members whose output starts within `want` bytes (at least min_round) of it, inflated
+// together; the vouched prefix becomes the held bytes. Returns -1 on a read or device error.
+int run_round(StreamFile* f, int64_t want) {
+  if (f->next_c > f->stage_off) {  // the stage keeps nothing behind the walk
+    const int64_t drop = std::min(f->next_c - f->stage_off, f->stage_len);
+    memmove(f->stage.p, f->stage.p + drop, (size_t)(f->stage_len - drop));
+    f->stage_off += drop;
+    f->stage_len -= drop;
+  }
+  const int64_t target = std::max(want, f->min_round);
+  const int64_t comp_cap = std::max(target, MIN_COMP_ROUND);
+  const size_t max_members = (size_t)std::max<int64_t>(64, comp_cap / MEMBERS_PER_BYTE);
+  std::vector<Member> ms;
+  int64_t out = 0, comp = 0, c = f->next_c;
+  int stop = 1;  // 1: the round is full; 2: the file ends at c; 0: the member at c is not for the walker
+  while (out < target && ms.size() < max_members) {
+    Member m;
+    const int r = walk_member(f, c, m);
+    if (r < 0) return -1;
+    if (r != 1) {
+      stop = r;
+      break;
+    }
+    if (!ms.empty() && comp + m.total > comp_cap) break;
+    m.out = out;
+    ms.push_back(m);
+    out += m.isize;
+    comp += m.total;
+    c += m.total;
+  }
+  int ok = 0;
+  if (!ms.empty()) {
+    if (!f->out.reserve((size_t)out + 1, 0)) {
+      f->error = "out of host memory for the BGZF output round";
+      return -1;
+    }
+    ok = f->device >= 0 ? inflate_device(f, ms, out) : inflate_host(f, ms);
+    if (ok < 0) return -1;
+  }
+  f->hold_b = 0;
+  if (ok < (int)ms.size()) {
+    f->hold_e = ms[ok].out;
+    f->next_c = f->fallback_c = ms[ok].c;
+  } else {
+    f->hold_e = out;
+    f->next_c = c;
+    if (stop == 0) f->fallback_c = c;
+    if (stop == 2) f->ended = true;
+  }
+  return 0;
+}
+
+int64_t read_walker(StreamFile* f, uint8_t* buf, size_t n) {
+  size_t got = 0;
+  while (got < n) {
+    if (f->hold_b < f->hold_e) {
+      const size_t k = std::min<size_t>(n - got, (size_t)(f->hold_e - f->hold_b));
+      memcpy(buf + got, f->out.p + f->hold_b, k);
+      f->hold_b += (int64_t)k;
+      got += k;
+      continue;
+    }
+    if (!f->tail && f->fallback_c >= 0) {
+      f->tail_pos = f->fallback_c;
+      f->tail.reset(new GzTail(
+          [f](uint8_t* b, size_t k) -> int64_t {
+            const int64_t staged = f->stage_off + f->stage_len - f->tail_pos;
+            if (staged > 0) {
+              const size_t m = std::min<size_t>(k, (size_t)staged);
+              memcpy(b, f->stage.p + (f->tail_pos - f->stage_off), m);
+              f->tail_pos += (int64_t)m;
+              return (int64_t)m;
+            }
+            if (f->file_eof) return 0;
+            for (;;) {
+              const ssize_t r = read(f->fd, b, k);
+              if (r < 0 && errno == EINTR) continue;
+              if (r < 0) return -1;
+              if (r == 0) f->file_eof = true;
+              f->cnt.compressed_bytes += r;
+              f->tail_pos += r;
+              return r;
+            }
+          },
+          f->tail_fresh));
+    }
+    if (f->tail) {
+      const int64_t r = f->tail->read(buf + got, n - got);
+      if (r < 0) return -1;
+      got += (size_t)r;
+      f->cnt.host_bytes += r;
+      break;
+    }
+    if (f->ended) break;
+    if (run_round(f, (int64_t)(n - got)) < 0) return -1;
+  }
+  return (int64_t)got;
+}
+
+}  // namespace
+
+StreamFile* open_stream(const char* path, bool force_gzread) {
+  std::unique_ptr<StreamFile> f(new StreamFile);
+  if (!force_gzread) {
+    f->fd = open(path, O_RDONLY);
+    if (f->fd < 0) return nullptr;
+    struct stat sb;
+    const bool regular = fstat(f->fd, &sb) == 0 && S_ISREG(sb.st_mode);
+    Member m;
+    const int r = walk_member(f.get(), 0, m);
+    if (r == 1) return f.release();
+    if (!regular && r >= 0) {  // a pipe: its first bytes are gone, so gzread is reproduced from them
+      f->fallback_c = 0;
+      f->tail_fresh = true;
+      return f.release();
+    }
+    close(f->fd);
+    f->fd = -1;
+    f->stage.release();
+    f->stage_len = 0;
+    f->file_eof = false;
+    f->cnt = StreamCounters();
+  }
   gzFile gz = gzopen(path, "rb");
   if (!gz) return nullptr;
-  gzbuffer(gz, 1 << 20);
-  StreamFile* f = new StreamFile;
+  gzbuffer(gz, GZ_BUFFER);
   f->gz = gz;
-  return f;
+  return f.release();
 }
 
-void close_stream(StreamFile* f) {
-  if (!f) return;
-  gzclose(f->gz);
-  delete f;
-}
+void close_stream(StreamFile* f) { delete f; }
 
 int64_t read_stream(StreamFile* f, void* buf, size_t n) {
+  if (f->fd >= 0) return read_walker(f, static_cast<uint8_t*>(buf), n);
   size_t got = 0;
   while (got < n) {
     const unsigned want = (unsigned)std::min<size_t>(n - got, 1u << 30);
@@ -111,10 +621,42 @@ int64_t read_stream(StreamFile* f, void* buf, size_t n) {
 }
 
 bool stream_truncated(StreamFile* f) {
+  if (f->fd >= 0) return f->tail && f->tail->truncated();
   int errnum = Z_OK;
   gzerror(f->gz, &errnum);
   return errnum != Z_OK;
 }
+
+bool bind_stream_device(StreamFile* f, int device, cudaStream_t stream, int64_t min_round) {
+  f->device = device;
+  f->st = stream;
+  f->min_round = min_round;
+  if (f->fd < 0) return true;
+  cudaError_t e = cudaSetDevice(device);
+  for (cudaEvent_t& ev : f->ev)
+    if (e == cudaSuccess && !ev) e = cudaEventCreate(&ev);
+  if (e != cudaSuccess) {
+    f->error = std::string("BGZF inflate: ") + cudaGetErrorString(e);
+    return false;
+  }
+  if (!f->stage.set_pinned((size_t)f->stage_len) || !f->out.set_pinned(0)) {
+    f->error = "BGZF inflate: out of page-locked host memory";
+    return false;
+  }
+  return true;
+}
+
+StreamCounters stream_counters(const StreamFile* f) {
+  StreamCounters c = f->cnt;
+  if (f->gz) c.compressed_bytes = (int64_t)gzoffset(f->gz);
+  return c;
+}
+
+size_t stream_device_bytes(const StreamFile* f) {
+  return f->d_comp.bytes() + f->d_out.bytes() + f->d_mem.bytes() + f->d_status.bytes();
+}
+
+const std::string& stream_error(const StreamFile* f) { return f->error; }
 
 void FastaText::release_text() {
   if (text) {
@@ -142,7 +684,8 @@ uint64_t concat_len_of(const std::vector<uint64_t>& lens) {
   return bytes * 2 - 1;
 }
 
-int read_fasta(const char* path, bool pinned, uint64_t max_concat_len, FastaText& out, std::string& err) {
+int read_fasta(const char* path, bool pinned, uint64_t max_concat_len, FastaText& out, std::string& err, int device,
+               cudaStream_t stream, StreamCounters* counters) {
   char msg[512];
   auto fail = [&](int rc, const char* fmt, const char* a = "", unsigned long long v = 0) {
     snprintf(msg, sizeof msg, fmt, a, v);
@@ -155,8 +698,15 @@ int read_fasta(const char* path, bool pinned, uint64_t max_concat_len, FastaText
   const long file_size = ftell(probe);
   fclose(probe);
   Input in;
+  auto read_failed = [&]() {
+    const std::string& e = stream_error(in.f);
+    err = std::string(path) + ": " + (e.empty() ? "read error (corrupt gzip stream?)" : e);
+    return -3;
+  };
   in.f = open_stream(path);
   if (!in.f) return fail(-2, "cannot open %s", path);
+  // a BGZF reference is inflated in rounds of at least 256 MiB: this reader asks for 16 KiB at a time
+  if (device >= 0 && !bind_stream_device(in.f, device, stream, 256ll << 20)) return read_failed();
   out.pinned = pinned;
   bool oom = false;
   // room for n more bytes of text: the file size for plain files, grown by doubling for compressed ones
@@ -259,11 +809,12 @@ int read_fasta(const char* path, bool pinned, uint64_t max_concat_len, FastaText
         break;
       }
     }
-    if (in.bad) return fail(-3, "%s: read error (corrupt gzip stream?)", path);
+    if (in.bad) return read_failed();
     out.recs.push_back(FastaRecord{name, start, len});
     if (len > 10) kept_bytes += (len + 1) / 2 + 500;
   }
-  if (in.bad) return fail(-3, "%s: read error (corrupt gzip stream?)", path);
+  if (in.bad) return read_failed();
+  if (counters) *counters = stream_counters(in.f);
   return 0;
 }
 

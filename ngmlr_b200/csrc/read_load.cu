@@ -451,7 +451,7 @@ struct ngmlr_b200_read_file {
            d_sp.owned_bytes() + d_qp.owned_bytes() + d_next_pos.owned_bytes() + d_scalar.owned_bytes() +
            d_ir.owned_bytes() + d_tr.owned_bytes() + d_stops.owned_bytes() + d_mark_segs.owned_bytes() +
            d_jump.owned_bytes() + d_rec_lines.owned_bytes() + d_count.owned_bytes() + d_recs.owned_bytes() +
-           d_layout.owned_bytes();
+           d_layout.owned_bytes() + stream_device_bytes(in);
   }
 };
 
@@ -494,7 +494,10 @@ int refill(ngmlr_b200_ctx* ctx, RF* f, bool grow) {
   if (!f->stream_eof) {
     const int64_t want = f->chunk_cap - f->n_host;
     const int64_t got = read_stream(f->in, f->h_chunk.p + f->n_host, (size_t)want);
-    if (got < 0) return ctx->fail("reads_load: %s: read error (corrupt gzip stream?)", f->path.c_str());
+    if (got < 0) {
+      const std::string& e = stream_error(f->in);
+      return ctx->fail("reads_load: %s: %s", f->path.c_str(), e.empty() ? "read error (corrupt gzip stream?)" : e.c_str());
+    }
     f->n_host += got;
     f->stream_bytes += got;
     if (got < want) {
@@ -743,6 +746,17 @@ int ngmlr_b200_read_file_stats(const ngmlr_b200_read_file* f, int64_t* stream_by
   return 0;
 }
 
+int ngmlr_b200_read_file_inflate_stats(const ngmlr_b200_read_file* f, int64_t* compressed_bytes,
+                                       int64_t* device_members, int64_t* host_bytes, float* inflate_ms) {
+  if (!f) return -1;
+  const StreamCounters c = stream_counters(f->in);
+  if (compressed_bytes) *compressed_bytes = c.compressed_bytes;
+  if (device_members) *device_members = c.device_members;
+  if (host_bytes) *host_bytes = c.host_bytes;
+  if (inflate_ms) *inflate_ms = c.inflate_ms;
+  return 0;
+}
+
 int ngmlr_b200_reads_load(ngmlr_b200_ctx* ctx, ngmlr_b200_read_file* f, int max_reads, int64_t max_bases,
                           int read_part_length, ngmlr_b200_sam_read* reads, int* n_reads, int* n_dropped) {
   if (!ctx) return -1;
@@ -754,6 +768,10 @@ int ngmlr_b200_reads_load(ngmlr_b200_ctx* ctx, ngmlr_b200_read_file* f, int max_
   *n_dropped = 0;
   if (f->device >= 0 && f->device != ctx->device) return ctx->fail("reads_load: the file is being read on another device");
   CU(cudaSetDevice(ctx->device));
+  if (f->device < 0 && !bind_stream_device(f->in, ctx->device, ctx->stream, 0)) {
+    f->error = "reads_load: " + f->path + ": " + stream_error(f->in);
+    return ctx->fail("%s", f->error.c_str());
+  }
   f->device = ctx->device;
   cudaStream_t st = ctx->stream;
   CsState* cs = cs_state(ctx, true);
@@ -837,6 +855,61 @@ int ngmlr_b200_reads_load(ngmlr_b200_ctx* ctx, ngmlr_b200_read_file* f, int max_
 }  // extern "C"
 
 extern "C" {
+
+// Test hook: the byte stream of a file as read_stream returns it in calls of read_size bytes, up to the first call
+// that returns less (or -1), under mode 0 = gzread, 1 = the stream layer without a device, 2 = the stream layer on
+// ctx's device and stream. Up to cap bytes are copied to out; *n_out = all bytes returned, *error = 1 when a call
+// returned -1, *truncated = stream_truncated afterwards, counters = {compressed bytes, device members, host
+// continuation bytes}, *inflate_ms the device kernel time. Returns 0, or < 0 when the file cannot be opened / bad
+// arguments / a CUDA error (message in ngmlr_b200_last_error(NULL)).
+int ngmlr_b200_debug_stream_read(const char* path, int mode, ngmlr_b200_ctx* ctx, int64_t read_size, uint8_t* out,
+                                 int64_t cap, int64_t* n_out, int32_t* error, int32_t* truncated, int64_t* counters,
+                                 float* inflate_ms) {
+  if (!path || read_size < 1 || mode < 0 || mode > 2 || (mode == 2 && !ctx)) {
+    set_error_without_context("debug_stream_read: bad arguments");
+    return -1;
+  }
+  StreamFile* f = open_stream(path, mode == 0);
+  if (!f) {
+    set_error_without_context(std::string("debug_stream_read: cannot open ") + path);
+    return -2;
+  }
+  if (mode == 2 && (cudaSetDevice(ctx->device) != cudaSuccess || !bind_stream_device(f, ctx->device, ctx->stream, 0))) {
+    set_error_without_context("debug_stream_read: " + stream_error(f));
+    close_stream(f);
+    return -3;
+  }
+  std::vector<uint8_t> buf((size_t)read_size);
+  int64_t total = 0;
+  int32_t err = 0;
+  for (;;) {
+    const int64_t r = read_stream(f, buf.data(), (size_t)read_size);
+    if (r < 0) {
+      err = 1;
+      if (!stream_error(f).empty()) {
+        set_error_without_context("debug_stream_read: " + stream_error(f));
+        close_stream(f);
+        return -3;
+      }
+      break;
+    }
+    if (out && total < cap) memcpy(out + total, buf.data(), (size_t)std::min(r, cap - total));
+    total += r;
+    if (r < read_size) break;
+  }
+  const StreamCounters c = stream_counters(f);
+  if (n_out) *n_out = total;
+  if (error) *error = err;
+  if (truncated) *truncated = stream_truncated(f);
+  if (counters) {
+    counters[0] = c.compressed_bytes;
+    counters[1] = c.device_members;
+    counters[2] = c.host_bytes;
+  }
+  if (inflate_ms) *inflate_ms = c.inflate_ms;
+  close_stream(f);
+  return 0;
+}
 
 // Test hook: the resident read set as the device holds it -- read offsets (n_reads + 1), read lengths, the sub-read
 // table (offsets, lengths; n_sub entries) and the arena bytes. Sizes always; arrays where not NULL.

@@ -64,6 +64,7 @@ int ngmlr_b200_load_reference(ngmlr_b200_ctx* ctx, const char* fasta_path, const
   const std::string idx_path =
       std::string(fasta_path) + "-ht-" + std::to_string(o.k) + "-" + std::to_string(o.kmer_skip) + ".2.ngm";
   int32_t fl = 0;
+  StreamCounters inflate;
   // ---- 1. the reference on the host: nothing on the context changes before it passed every check ----
   FastaText fa;
   PinBuf<uint8_t> enc_host;
@@ -98,7 +99,9 @@ int ngmlr_b200_load_reference(ngmlr_b200_ctx* ctx, const char* fasta_path, const
     fl |= NGMLR_B200_LOAD_REFERENCE_READ;
   } else {
     std::string err;
-    if (read_fasta(fasta_path, true, INDEX_MAX_CONCAT_LEN, fa, err) != 0) return ctx->fail("load_reference: %s", err.c_str());
+    CU(cudaSetDevice(ctx->device));
+    if (read_fasta(fasta_path, true, INDEX_MAX_CONCAT_LEN, fa, err, ctx->device, ctx->stream, &inflate) != 0)
+      return ctx->fail("load_reference: %s", err.c_str());
     std::vector<uint64_t> all;
     for (const FastaRecord& r : fa.recs) {
       all.push_back(r.len);
@@ -217,6 +220,7 @@ int ngmlr_b200_load_reference(ngmlr_b200_ctx* ctx, const char* fasta_path, const
   const float ms[6] = {(float)(t1 - t0), (float)(t2 - t1), (float)(t3 - t2), (float)((idx_cached ? t4a : t5) - t3),
                        (float)(t6 - (idx_cached ? t4a : t5)), (float)(t6 - t0)};
   memcpy(cs->load_ms, ms, sizeof ms);
+  cs->load_inflate = inflate;
   if (n_contigs) *n_contigs = (int32_t)starts.size();
   if (concat_len) *concat_len = cs->concat_len;
   if (flags) *flags = fl;
@@ -247,6 +251,22 @@ int ngmlr_b200_load_reference_ms(ngmlr_b200_ctx* ctx, float* ms) {
   CsState* cs = cs_state(ctx, false);
   if (!cs) return ctx->fail("load_reference_ms: no load");
   memcpy(ms, cs->load_ms, sizeof cs->load_ms);
+  return 0;
+}
+
+// What inflating the FASTA file of the context's last load_reference did (all 0 when the caches were read or the
+// file is not compressed): bytes read from the file, BGZF members inflated on the device, bytes inflated by the host
+// continuation, device inflate milliseconds. Any pointer may be NULL.
+int ngmlr_b200_load_reference_inflate_stats(ngmlr_b200_ctx* ctx, int64_t* compressed_bytes, int64_t* device_members,
+                                            int64_t* host_bytes, float* inflate_ms) {
+  if (!ctx) return -1;
+  CsState* cs = cs_state(ctx, false);
+  if (!cs) return ctx->fail("load_reference_inflate_stats: no load");
+  const StreamCounters& c = cs->load_inflate;
+  if (compressed_bytes) *compressed_bytes = c.compressed_bytes;
+  if (device_members) *device_members = c.device_members;
+  if (host_bytes) *host_bytes = c.host_bytes;
+  if (inflate_ms) *inflate_ms = c.inflate_ms;
   return 0;
 }
 

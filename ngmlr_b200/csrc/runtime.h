@@ -20,6 +20,7 @@
 #include "../../include/ngmlr_b200.h"
 #include "cigar_text.h"
 #include "device_types.h"
+#include "fasta.h"
 #include "kernels.h"
 
 namespace nb {
@@ -438,6 +439,7 @@ struct CsState {
   std::vector<const char*> contig_name_ptrs;
   std::vector<uint64_t> contig_start, contig_len;
   float load_ms[6] = {0, 0, 0, 0, 0, 0};  // read / parse, install, reference write, index, index write, total
+  StreamCounters load_inflate;            // the FASTA file's inflate in the last load_reference
 };
 
 CsState* cs_state(ngmlr_b200_ctx* ctx, bool create);

@@ -4,7 +4,10 @@ card's name and power limit read in the same run and the peak device memory in u
 it runs the reference's own build (ref_cs_init_save of oracle/_ref/libngmlr_full.so) and the device load on a smaller
 genome (--cpu-mbp) that the CPU build finishes in reasonable time.
 
-    python scripts/index_timing.py [--gbp 3] [--contigs 24] [--cpu-mbp 50] [--out DIR]
+    python scripts/index_timing.py [--gbp 3] [--contigs 24] [--cpu-mbp 50] [--compressed] [--out DIR]
+
+--compressed also loads the same genome as BGZF (inflated on the device) and as multi-member gzip (gzread on one host
+thread), both level 6 and written by a process pool, with their read phase and inflate counters.
 
 Phase times are host clocks around work that ends in a device synchronise (ngmlr_b200_load_reference_ms); the device
 index build alone is also timed with CUDA events (ngmlr_b200_cs_last_build_ms)."""
@@ -84,6 +87,8 @@ def load(path, gpu):
         done.set()
         th.join()
     return {"contigs": len(ref.names), "positions": ref.concat_len, "phases_ms": ref.ms, "wall_ms_with_context": wall,
+            "inflate": {"compressed_bytes_read": ref.compressed_bytes, "device_members": ref.device_members,
+                        "host_inflated_bytes": ref.host_bytes, "inflate_kernel_ms": ref.inflate_ms},
             "index_build_kernel_ms_cuda_events": build_ms,
             "files": {"reference_written": ref.reference_written, "index_written": ref.index_written},
             "device_mem_in_use_before_GB": (total - free0) / 1e9, "device_mem_in_use_peak_GB": peak[0] / 1e9,
@@ -104,6 +109,7 @@ def main():
     ap.add_argument("--cpu-mbp", type=float, default=50.0)
     ap.add_argument("--gpu", type=int, default=0)
     ap.add_argument("--seed", type=int, default=1)
+    ap.add_argument("--compressed", action="store_true", help="also load BGZF and gzip copies of the genome")
     ap.add_argument("--out", default=None, help="also write the JSON result here")
     a = ap.parse_args()
     out = {"gpu": gpu_info()}
@@ -115,6 +121,19 @@ def main():
         out["genome_write_s"] = time.perf_counter() - t0
         out["fasta_bytes"] = os.path.getsize(big)
         out["device_load"] = load(big, a.gpu)
+        if a.compressed:
+            sys.path.insert(0, os.path.join(ROOT, "tests"))
+            import bgzf_cases as B
+            for name, blocked in (("bgzf", True), ("gzip", False)):
+                path = os.path.join(work, "genome_" + name + ".fa.gz")
+                t0 = time.perf_counter()
+                size = B.compress_file(big, path, 6, blocked)
+                out[name + "_compress_s"] = time.perf_counter() - t0
+                out[name + "_bytes"] = size
+                out[name + "_device_load"] = load(path, a.gpu)
+                for f in os.listdir(work):
+                    if f.startswith("genome_"):
+                        os.remove(os.path.join(work, f))
         for f in os.listdir(work):
             os.remove(os.path.join(work, f))
         small = os.path.join(work, "small.fa")

@@ -1,12 +1,13 @@
 """Read loading speed: ngmlr_b200_reads_load (B200Aligner.load_reads) on a synthetic FASTQ shaped like bench.py's
-pacbio50 reads (lognormal lengths, median 8 000, at most 40 000 bases; 4-line records, Phred+33 qualities), plain and
-gzip, next to the unmodified ReadProvider on one thread (ref_read_file of oracle/_ref/libngmlr_reads.so, where built).
+pacbio50 reads (lognormal lengths, median 8 000, at most 40 000 bases; 4-line records, Phred+33 qualities), plain,
+gzip and BGZF (level 6, compressed by a process pool; inflated on the device), next to the unmodified ReadProvider on
+one thread (ref_read_file of oracle/_ref/libngmlr_reads.so, where built).
 
-Reports GB/s of stream text and Gbp/s of bases for each, the host read / inflate, device parse and gather phases, and
-the peak device memory of the run (cudaMemGetInfo sampled after every batch, less the level before the first load).
-Prints one JSON object, and writes it to --out where given.
+Reports GB/s of stream text and Gbp/s of bases for each, the host read / inflate, device parse and gather phases, the
+device inflate kernel's own GB/s of output (CUDA events), and the peak device memory of the run (cudaMemGetInfo sampled
+after every batch, less the level before the first load). Prints one JSON object, and writes it to --out where given.
 
-    python scripts/read_load_timing.py --gb 4 [--gzip-gb 1] [--oracle-gb 0.5]"""
+    python scripts/read_load_timing.py --gb 4 [--gzip-gb 1] [--bgzf-gb 4] [--oracle-gb 0.5]"""
 import argparse
 import ctypes as C
 import gzip
@@ -89,10 +90,17 @@ def time_native(path, chunk_bytes, max_bases):
     ms = [C.c_float(0) for _ in range(3)]
     lib.ngmlr_b200_read_file_stats(f, C.byref(sb), C.byref(rc), C.byref(ms[0]), C.byref(ms[1]), C.byref(ms[2]),
                                    C.byref(dev))
+    cb, dm, hb, ims = C.c_int64(0), C.c_int64(0), C.c_int64(0), C.c_float(0)
+    lib.ngmlr_b200_read_file_inflate_stats(f, C.byref(cb), C.byref(dm), C.byref(hb), C.byref(ims))
     lib.ngmlr_b200_read_file_close(f)
     a.close()
-    return dict(seconds=dt, reads=total, gb_per_s=sb.value / dt / 1e9, read_ms=ms[0].value, parse_ms=ms[1].value,
-                gather_ms=ms[2].value, handle_device_bytes=dev.value)
+    res = dict(seconds=dt, reads=total, gb_per_s=sb.value / dt / 1e9, read_ms=ms[0].value, parse_ms=ms[1].value,
+               gather_ms=ms[2].value, handle_device_bytes=dev.value, compressed_bytes_read=cb.value,
+               device_members=dm.value, host_inflated_bytes=hb.value, inflate_kernel_ms=ims.value)
+    if ims.value > 0:
+        res["inflate_kernel_gb_per_s"] = sb.value / ims.value / 1e6
+        res["inflate_kernel_share_of_load"] = ims.value / (dt * 1e3)
+    return res
 
 
 def time_oracle(path, stream_bytes, bases):
@@ -113,6 +121,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gb", type=float, default=4.0, help="plain FASTQ size")
     ap.add_argument("--gzip-gb", type=float, default=1.0, help="FASTQ size (uncompressed) of the gzip run")
+    ap.add_argument("--bgzf-gb", type=float, default=4.0, help="FASTQ size (uncompressed) of the BGZF run")
     ap.add_argument("--oracle-gb", type=float, default=0.5, help="FASTQ size of the ReadProvider run")
     ap.add_argument("--chunk-mb", type=int, default=256)
     ap.add_argument("--max-bases", type=int, default=200_000_000)
@@ -132,10 +141,23 @@ def main():
     time_loader(plain, sb, bases, chunk, args.max_bases)  # page cache and module load
     res["plain"] = time_loader(plain, sb, bases, chunk, args.max_bases)
     res["plain_native"] = time_native(plain, chunk, args.max_bases)
+    if args.bgzf_gb > 0:
+        import bgzf_cases as B
+        if args.bgzf_gb != args.gb:
+            os.unlink(plain)
+            sb, bases, _ = write_fastq(plain, args.bgzf_gb)
+        bz = os.path.join(d, "reads.fq.bgz")
+        t0 = time.perf_counter()
+        res["bgzf_file"] = dict(bytes=sb, compressed_bytes=B.compress_file(plain, bz, 6),
+                                compress_seconds=time.perf_counter() - t0)
+        res["bgzf_native"] = time_native(bz, chunk, args.max_bases)
+        res["bgzf"] = time_loader(bz, sb, bases, chunk, args.max_bases)
+        os.unlink(bz)
     os.unlink(plain)
     gz = os.path.join(d, "reads.fq.gz")
     gsb, gbases, _ = write_fastq(gz, args.gzip_gb, seed=2, opener=lambda p, m: gzip.open(p, m, compresslevel=1))
     res["gzip"] = time_loader(gz, gsb, gbases, chunk, args.max_bases)
+    res["gzip_native"] = time_native(gz, chunk, args.max_bases)
     res["gzip"]["compressed_bytes"] = os.path.getsize(gz)
     os.unlink(gz)
     if args.oracle_gb > 0:
