@@ -553,9 +553,12 @@ int ngmlr_b200_map_short_reads(ngmlr_b200_ctx* ctx, int read_part_length, float 
  * first member the device cannot vouch for (anything zlib would refuse or read differently), and for every other gzip
  * file, zlib inflates on the calling thread exactly as gzread does. Each chunk goes to the device once: its line
  * table, the record structure (kseq's rules, multi-line FASTQ and quality lines starting with '@' / '>' included) and
- * the normalised bases are computed there. Device memory of a handle stays below 9 x chunk_bytes, and for BGZF input
- * (which adds the compressed staging and the inflated output of a round) below 11 x max(chunk_bytes, 1 MiB). No
- * reference counterpart for the handle itself. */
+ * the normalised bases are computed there. A chunk's line table holds at most max(capacity / 32, 4096) lines; a chunk
+ * with more newlines is resolved up to the last newline the table holds and the rest moves to the next chunk. The
+ * chunk's capacity starts at chunk_bytes and doubles whenever its first record does not fit in its bytes or its line
+ * table. Device memory of a handle stays below 9 x max(capacity, 128 KiB), with the capacity as it has grown, and for
+ * BGZF input (which adds the compressed staging and the inflated output of a round) below 11 x max(capacity, 1 MiB).
+ * No reference counterpart for the handle itself. */
 typedef struct ngmlr_b200_read_file ngmlr_b200_read_file;
 typedef struct {
   int64_t chunk_bytes; /* page-locked staging per chunk; 0 = 256 MiB; grows for a larger record */
@@ -588,6 +591,10 @@ int ngmlr_b200_read_file_stats(const ngmlr_b200_read_file* f, int64_t* stream_by
  * of the device inflate kernel (CUDA events). Any pointer may be NULL. */
 int ngmlr_b200_read_file_inflate_stats(const ngmlr_b200_read_file* f, int64_t* compressed_bytes,
                                        int64_t* device_members, int64_t* host_bytes, float* inflate_ms);
+/* Test hook: how the handle's chunks went so far -- chunks resolved, chunks cut short at a full line table, chunk
+ * doublings, and the chunk capacity in bytes now. Any pointer may be NULL. */
+int ngmlr_b200_debug_read_file_chunks(const ngmlr_b200_read_file* f, int64_t* chunks, int64_t* line_limited,
+                                      int64_t* grows, int64_t* chunk_cap);
 
 #ifdef __cplusplus
 }

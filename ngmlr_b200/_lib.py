@@ -71,6 +71,7 @@ C_API_SYMBOLS = (
     "ngmlr_b200_map_short_reads", "ngmlr_b200_load_reference", "ngmlr_b200_reference_contigs",
     "ngmlr_b200_read_file_open", "ngmlr_b200_read_file_close", "ngmlr_b200_reads_load", "ngmlr_b200_reads_load_dropped",
     "ngmlr_b200_read_file_stats", "ngmlr_b200_read_file_inflate_stats", "ngmlr_b200_load_reference_inflate_stats",
+    "ngmlr_b200_debug_read_file_chunks",
 )
 
 # flags of ngmlr_b200_load_reference (include/ngmlr_b200.h)
@@ -195,6 +196,7 @@ def load():
     f32p = C.POINTER(C.c_float)
     lib.ngmlr_b200_read_file_stats.argtypes = [vp, i64p, i64p, f32p, f32p, f32p, i64p]
     lib.ngmlr_b200_read_file_inflate_stats.argtypes = [vp, i64p, i64p, i64p, f32p]
+    lib.ngmlr_b200_debug_read_file_chunks.argtypes = [vp, i64p, i64p, i64p, i64p]
     lib.ngmlr_b200_load_reference_inflate_stats.argtypes = [vp, i64p, i64p, i64p, f32p]
     lib.ngmlr_b200_debug_stream_read.argtypes = [C.c_char_p, C.c_int, vp, C.c_int64, vp, C.c_int64, i64p, i32p, i32p,
                                                  i64p, f32p]

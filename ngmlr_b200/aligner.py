@@ -221,7 +221,9 @@ class ReadBatch:
     """One ngmlr_b200_reads_load call: samtext.Read records, the number of sub-reads of the resident set, and the name
     of a read ngmlr would have dropped (quality length differs from the sequence length; it ends the file). The inflate
     counters are the handle's so far: bytes read from the file, BGZF members inflated on the device, bytes inflated by
-    the host continuation, device inflate milliseconds."""
+    the host continuation, device inflate milliseconds. So are the chunk counters: records resolved, the most device
+    memory the handle held, chunks resolved, chunks cut short at a full line table, chunk doublings and the chunk
+    capacity in bytes now."""
     reads: list
     n_sub: int
     dropped: list
@@ -229,6 +231,12 @@ class ReadBatch:
     device_members: int = 0
     host_bytes: int = 0
     inflate_ms: float = 0.0
+    records: int = 0
+    device_bytes: int = 0
+    chunks: int = 0
+    line_limited: int = 0
+    grows: int = 0
+    chunk_cap: int = 0
 
 
 class B200Aligner:
@@ -536,7 +544,12 @@ class B200Aligner:
                 if reads or dropped:
                     cb, dm, hb, ims = C.c_int64(0), C.c_int64(0), C.c_int64(0), C.c_float(0)
                     self.lib.ngmlr_b200_read_file_inflate_stats(f, C.byref(cb), C.byref(dm), C.byref(hb), C.byref(ims))
-                    yield ReadBatch(reads, n_sub, dropped, cb.value, dm.value, hb.value, float(ims.value))
+                    recs_n, dev = C.c_int64(0), C.c_int64(0)
+                    self.lib.ngmlr_b200_read_file_stats(f, None, C.byref(recs_n), None, None, None, C.byref(dev))
+                    ch = [C.c_int64(0) for _ in range(4)]
+                    self.lib.ngmlr_b200_debug_read_file_chunks(f, *[C.byref(x) for x in ch])
+                    yield ReadBatch(reads, n_sub, dropped, cb.value, dm.value, hb.value, float(ims.value), recs_n.value,
+                                    dev.value, *[x.value for x in ch])
                 if n.value == 0:
                     break
         finally:

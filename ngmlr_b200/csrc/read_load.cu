@@ -444,6 +444,7 @@ struct ngmlr_b200_read_file {
   PinBuf<uint8_t> h_seq;
   std::vector<std::string> quals;
   int64_t records = 0, device_peak = 0;
+  int64_t chunks = 0, line_limited = 0, grows = 0;  // chunks resolved, of them cut at a full line table; doublings
   float read_ms = 0, parse_ms = 0, gather_ms = 0;
   size_t device_bytes() const {
     return d_chunk.owned_bytes() + d_tmp.owned_bytes() + d_fb.owned_bytes() + d_stop_flag.owned_bytes() +
@@ -483,7 +484,10 @@ int refill(ngmlr_b200_ctx* ctx, RF* f, bool grow) {
   if (keep > 0 && f->tail > 0) memmove(f->h_chunk.p, f->h_chunk.p + f->tail, (size_t)keep);
   f->n_host = keep;
   f->tail = 0;
-  if (grow) f->chunk_cap *= 2;
+  if (grow) {
+    f->chunk_cap *= 2;
+    ++f->grows;
+  }
   if ((int64_t)f->h_chunk.cap < f->chunk_cap + 1) {
     PinBuf<uint8_t> nb_;
     RCU(nb_.reserve((size_t)f->chunk_cap + 1));
@@ -546,6 +550,8 @@ int resolve_chunk(ngmlr_b200_ctx* ctx, RF* f) {
   if (total_nl > limit) n_res = last_nl + 1;
   const int n_lines = n_nl + (n_res > last_nl + 1 ? 1 : 0);
   f->n_res = n_res;
+  ++f->chunks;
+  if (n_res < n) ++f->line_limited;
   Chunk& k = f->k;
   k = Chunk{};
   k.c = f->d_chunk.p;
@@ -743,6 +749,16 @@ int ngmlr_b200_read_file_stats(const ngmlr_b200_read_file* f, int64_t* stream_by
   if (parse_ms) *parse_ms = f->parse_ms;
   if (gather_ms) *gather_ms = f->gather_ms;
   if (device_bytes) *device_bytes = f->device_peak;
+  return 0;
+}
+
+int ngmlr_b200_debug_read_file_chunks(const ngmlr_b200_read_file* f, int64_t* chunks, int64_t* line_limited,
+                                      int64_t* grows, int64_t* chunk_cap) {
+  if (!f) return -1;
+  if (chunks) *chunks = f->chunks;
+  if (line_limited) *line_limited = f->line_limited;
+  if (grows) *grows = f->grows;
+  if (chunk_cap) *chunk_cap = f->chunk_cap;
   return 0;
 }
 

@@ -113,13 +113,13 @@ def _ngmlr_sam(ref_dir, query, out, rpl):
     return [l for l in open(out, "rb").read().split(b"\n") if l and not l.startswith(b"@")]
 
 
-def _library_sam(tmp_path, query, rpl):
+def _library_sam(tmp_path, query, rpl, chunk_bytes=0):
     ref = shutil.copyfile(os.path.join(FIX, "ref_chr21_20kb.fa"), str(tmp_path / "lib_ref.fa"))
     a = B200Aligner(0)
     try:
         loaded = a.load_reference(ref, skip_write=True)
         out = b""
-        for batch in a.load_reads(query, read_part_length=rpl, max_reads=500):
+        for batch in a.load_reads(query, read_part_length=rpl, max_reads=500, chunk_bytes=chunk_bytes):
             a.cs_run(read_part_length=rpl)
             res = a.map_short_reads(read_part_length=rpl)
             recs = [samtext.Read(r.name, r.seq, r.qual, m[1], m[0], r.empty) for r, m in zip(batch.reads, res)]
