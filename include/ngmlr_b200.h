@@ -430,6 +430,10 @@ int ngmlr_b200_reference_contigs(ngmlr_b200_ctx* ctx, const char** names, int32_
  * may be NULL. Returns 0 or < 0. */
 int ngmlr_b200_load_reference_inflate_stats(ngmlr_b200_ctx* ctx, int64_t* compressed_bytes, int64_t* device_members,
                                             int64_t* host_bytes, float* inflate_ms);
+/* What the plain gzip path did in the last load_reference (see ngmlr_b200_read_file_gzip_stats); all 0 unless the
+ * FASTA file was a gzip file whose first member is not BGZF. Any pointer may be NULL. Returns 0 or < 0. */
+int ngmlr_b200_load_reference_gzip_stats(ngmlr_b200_ctx* ctx, int64_t* device_bytes, int64_t* chunks,
+                                         int64_t* redecoded, float* kernel_ms);
 
 /* ---- SAM text (SURVEY section 8(f)4) ----------------------------------------------------------
  * Replaces SAMWriter::DoWriteProlog / DoWriteRead -> DoWriteReadGeneric / DoWriteUnmappedRead
@@ -549,15 +553,21 @@ int ngmlr_b200_map_short_reads(ngmlr_b200_ctx* ctx, int read_part_length, float 
  * IParser::copyToRead (src/ReadProvider.cpp:136-187, src/IParser.h:51-117), parsed on the device ------------------
  * The file is read in chunks of chunk_bytes (0: 256 MiB) into page-locked memory; a chunk too small for one record
  * grows. Compressed input: a BGZF file (first member header 1f 8b 08, FLG 0x04 with a BC extra subfield, as bgzip /
- * htslib write it) is inflated on the context's device, one warp per member, from the first reads_load on; from the
- * first member the device cannot vouch for (anything zlib would refuse or read differently), and for every other gzip
- * file, zlib inflates on the calling thread exactly as gzread does. Each chunk goes to the device once: its line
+ * htslib write it) is inflated on the context's device, one warp per member, from the first reads_load on. Any other
+ * gzip file (gzip, pigz, Python's gzip: one deflate stream per member) is inflated on the device too, in rounds of
+ * speculative chunks whose block starts are found by testing every bit offset and confirmed along the decode chain,
+ * when it is a regular file read in chunks of at least 256 MiB and its compression ratio is one at which the device
+ * beats zlib (DESIGN.md §4.9).
+ * From the first member the device cannot vouch for (anything zlib would refuse or read differently), zlib inflates
+ * on the calling thread exactly as gzread does. Each chunk goes to the device once: its line
  * table, the record structure (kseq's rules, multi-line FASTQ and quality lines starting with '@' / '>' included) and
  * the normalised bases are computed there. A chunk's line table holds at most max(capacity / 32, 4096) lines; a chunk
  * with more newlines is resolved up to the last newline the table holds and the rest moves to the next chunk. The
  * chunk's capacity starts at chunk_bytes and doubles whenever its first record does not fit in its bytes or its line
  * table. Device memory of a handle stays below 9 x max(capacity, 128 KiB), with the capacity as it has grown, and for
- * BGZF input (which adds the compressed staging and the inflated output of a round) below 11 x max(capacity, 1 MiB).
+ * BGZF input (which adds the compressed staging and the inflated output of a round) below 11 x max(capacity, 1 MiB),
+ * and for other gzip input (which adds the compressed span, 16-bit speculative and byte output of a round, per-chunk
+ * tables and the 32 KiB window) below 13 x max(capacity, 1 MiB) + 48 MiB.
  * No reference counterpart for the handle itself. */
 typedef struct ngmlr_b200_read_file ngmlr_b200_read_file;
 typedef struct {
@@ -591,6 +601,11 @@ int ngmlr_b200_read_file_stats(const ngmlr_b200_read_file* f, int64_t* stream_by
  * of the device inflate kernel (CUDA events). Any pointer may be NULL. */
 int ngmlr_b200_read_file_inflate_stats(const ngmlr_b200_read_file* f, int64_t* compressed_bytes,
                                        int64_t* device_members, int64_t* host_bytes, float* inflate_ms);
+/* What the plain gzip path (any gzip file whose first member is not BGZF) did for the handle so far: bytes it
+ * returned from the device, chunks placed, chunks decoded again after a chain mismatch (a false block start costs
+ * time, never bytes) and kernel milliseconds. Any pointer may be NULL. */
+int ngmlr_b200_read_file_gzip_stats(const ngmlr_b200_read_file* f, int64_t* device_bytes, int64_t* chunks,
+                                    int64_t* redecoded, float* kernel_ms);
 /* Test hook: how the handle's chunks went so far -- chunks resolved, chunks cut short at a full line table, chunk
  * doublings, and the chunk capacity in bytes now. Any pointer may be NULL. */
 int ngmlr_b200_debug_read_file_chunks(const ngmlr_b200_read_file* f, int64_t* chunks, int64_t* line_limited,

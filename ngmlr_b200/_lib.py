@@ -71,6 +71,7 @@ C_API_SYMBOLS = (
     "ngmlr_b200_map_short_reads", "ngmlr_b200_load_reference", "ngmlr_b200_reference_contigs",
     "ngmlr_b200_read_file_open", "ngmlr_b200_read_file_close", "ngmlr_b200_reads_load", "ngmlr_b200_reads_load_dropped",
     "ngmlr_b200_read_file_stats", "ngmlr_b200_read_file_inflate_stats", "ngmlr_b200_load_reference_inflate_stats",
+    "ngmlr_b200_read_file_gzip_stats", "ngmlr_b200_load_reference_gzip_stats",
     "ngmlr_b200_debug_read_file_chunks",
 )
 
@@ -200,6 +201,10 @@ def load():
     lib.ngmlr_b200_load_reference_inflate_stats.argtypes = [vp, i64p, i64p, i64p, f32p]
     lib.ngmlr_b200_debug_stream_read.argtypes = [C.c_char_p, C.c_int, vp, C.c_int64, vp, C.c_int64, i64p, i32p, i32p,
                                                  i64p, f32p]
+    lib.ngmlr_b200_read_file_gzip_stats.argtypes = [vp, i64p, i64p, i64p, f32p]
+    lib.ngmlr_b200_load_reference_gzip_stats.argtypes = [vp, i64p, i64p, i64p, f32p]
+    lib.ngmlr_b200_debug_gzip_stream_read.argtypes = [C.c_char_p, vp, C.c_int64, C.c_int64, vp, C.c_int64, i64p, i32p,
+                                                      i32p, i64p, i64p]
     lib.ngmlr_b200_debug_resident_reads.argtypes = [vp, i32p, i32p, i64p, vp, vp, vp, vp, vp]
     lib.ngmlr_b200_sw_last_kernel_ms.argtypes = [vp]
     lib.ngmlr_b200_sw_last_kernel_ms.restype = C.c_float

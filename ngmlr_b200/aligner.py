@@ -42,6 +42,12 @@ class LoadedReference:
     device_members: int = 0
     host_bytes: int = 0
     inflate_ms: float = 0.0
+    # the plain gzip path (a gzip file whose first member is not BGZF): bytes it returned from the device, chunks
+    # placed, chunks decoded again after a chain mismatch, kernel milliseconds
+    gzip_bytes: int = 0
+    gzip_chunks: int = 0
+    gzip_redecoded: int = 0
+    gzip_ms: float = 0.0
 
     def sam_ref_names(self):
         """The reference list SAM records index (ids count both strands): every name twice."""
@@ -223,7 +229,8 @@ class ReadBatch:
     counters are the handle's so far: bytes read from the file, BGZF members inflated on the device, bytes inflated by
     the host continuation, device inflate milliseconds. So are the chunk counters: records resolved, the most device
     memory the handle held, chunks resolved, chunks cut short at a full line table, chunk doublings and the chunk
-    capacity in bytes now."""
+    capacity in bytes now. So are the plain gzip counters: bytes returned from the device, chunks placed, chunks
+    decoded again after a chain mismatch, kernel milliseconds."""
     reads: list
     n_sub: int
     dropped: list
@@ -237,6 +244,10 @@ class ReadBatch:
     line_limited: int = 0
     grows: int = 0
     chunk_cap: int = 0
+    gzip_bytes: int = 0
+    gzip_chunks: int = 0
+    gzip_redecoded: int = 0
+    gzip_ms: float = 0.0
 
 
 class B200Aligner:
@@ -404,12 +415,16 @@ class B200Aligner:
         cb, dm, hb, ims = C.c_int64(0), C.c_int64(0), C.c_int64(0), C.c_float(0)
         self._check(self.lib.ngmlr_b200_load_reference_inflate_stats(self.h, C.byref(cb), C.byref(dm), C.byref(hb),
                                                                       C.byref(ims)))
+        gb, gc, gr, gms = C.c_int64(0), C.c_int64(0), C.c_int64(0), C.c_float(0)
+        self._check(self.lib.ngmlr_b200_load_reference_gzip_stats(self.h, C.byref(gb), C.byref(gc), C.byref(gr),
+                                                                   C.byref(gms)))
         return LoadedReference([names[i][:int(nlen[i])] for i in range(n.value)], [int(x) for x in starts],
                                [int(x) for x in lens], int(cl.value),
                                bool(f & _lib.LOAD_REFERENCE_READ), bool(f & _lib.LOAD_REFERENCE_WRITTEN),
                                bool(f & _lib.LOAD_INDEX_READ), bool(f & _lib.LOAD_INDEX_WRITTEN),
                                dict(zip(LoadedReference.PHASES, [float(x) for x in ms])),
-                               cb.value, dm.value, hb.value, float(ims.value))
+                               cb.value, dm.value, hb.value, float(ims.value), gb.value, gc.value, gr.value,
+                               float(gms.value))
 
     def set_reference(self, ref):
         """ref: ngmlr_b200.refindex.EncodedReference (the reference's 4-bit `binRef`)."""
@@ -548,8 +563,10 @@ class B200Aligner:
                     self.lib.ngmlr_b200_read_file_stats(f, None, C.byref(recs_n), None, None, None, C.byref(dev))
                     ch = [C.c_int64(0) for _ in range(4)]
                     self.lib.ngmlr_b200_debug_read_file_chunks(f, *[C.byref(x) for x in ch])
+                    gz = [C.c_int64(0) for _ in range(3)] + [C.c_float(0)]
+                    self.lib.ngmlr_b200_read_file_gzip_stats(f, *[C.byref(x) for x in gz])
                     yield ReadBatch(reads, n_sub, dropped, cb.value, dm.value, hb.value, float(ims.value), recs_n.value,
-                                    dev.value, *[x.value for x in ch])
+                                    dev.value, *[x.value for x in ch], *[x.value for x in gz])
                 if n.value == 0:
                     break
         finally:

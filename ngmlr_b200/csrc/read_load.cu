@@ -2,7 +2,8 @@
 //
 // ngmlr reads its query file with ReadProvider::NextRead -> FastXParser -> kseq_read -> IParser::copyToRead
 // (src/ReadProvider.cpp:136-187, src/IParser.h:51-117, src/kseq.h:171-211) on one thread under GetNextReadBatch's
-// mutex. Here a chunk of the byte stream (plain, or inflated by zlib on the host) goes to the device once and:
+// mutex. Here a chunk of the byte stream (plain, or inflated on the device or by zlib on the host: fasta.cpp) goes to
+// the device once and:
 //   1. line table: one warp per 2 KiB segment counts '\n' with ballots; a scan gives every newline its rank and a
 //      second pass writes the positions. The same pass notes each segment's first '>' / '@' byte.
 //   2. per line: first byte, trailing '\r' count, and what the line adds to a sequence and to a quality string under
@@ -773,6 +774,17 @@ int ngmlr_b200_read_file_inflate_stats(const ngmlr_b200_read_file* f, int64_t* c
   return 0;
 }
 
+int ngmlr_b200_read_file_gzip_stats(const ngmlr_b200_read_file* f, int64_t* device_bytes, int64_t* chunks,
+                                    int64_t* redecoded, float* kernel_ms) {
+  if (!f) return -1;
+  const StreamCounters c = stream_counters(f->in);
+  if (device_bytes) *device_bytes = c.gzip_bytes;
+  if (chunks) *chunks = c.gzip_chunks;
+  if (redecoded) *redecoded = c.gzip_redecoded;
+  if (kernel_ms) *kernel_ms = c.gzip_ms;
+  return 0;
+}
+
 int ngmlr_b200_reads_load(ngmlr_b200_ctx* ctx, ngmlr_b200_read_file* f, int max_reads, int64_t max_bases,
                           int read_part_length, ngmlr_b200_sam_read* reads, int* n_reads, int* n_dropped) {
   if (!ctx) return -1;
@@ -878,9 +890,9 @@ extern "C" {
 // returned -1, *truncated = stream_truncated afterwards, counters = {compressed bytes, device members, host
 // continuation bytes}, *inflate_ms the device kernel time. Returns 0, or < 0 when the file cannot be opened / bad
 // arguments / a CUDA error (message in ngmlr_b200_last_error(NULL)).
-int ngmlr_b200_debug_stream_read(const char* path, int mode, ngmlr_b200_ctx* ctx, int64_t read_size, uint8_t* out,
-                                 int64_t cap, int64_t* n_out, int32_t* error, int32_t* truncated, int64_t* counters,
-                                 float* inflate_ms) {
+static int debug_stream(const char* path, int mode, ngmlr_b200_ctx* ctx, int64_t read_size, int64_t gzip_chunk,
+                        uint8_t* out, int64_t cap, int64_t* n_out, int32_t* error, int32_t* truncated,
+                        int64_t* counters, float* inflate_ms, int64_t* gzip) {
   if (!path || read_size < 1 || mode < 0 || mode > 2 || (mode == 2 && !ctx)) {
     set_error_without_context("debug_stream_read: bad arguments");
     return -1;
@@ -895,6 +907,7 @@ int ngmlr_b200_debug_stream_read(const char* path, int mode, ngmlr_b200_ctx* ctx
     close_stream(f);
     return -3;
   }
+  if (mode == 2 && gzip_chunk > 0) set_gzip_chunk(f, gzip_chunk);
   std::vector<uint8_t> buf((size_t)read_size);
   int64_t total = 0;
   int32_t err = 0;
@@ -923,8 +936,30 @@ int ngmlr_b200_debug_stream_read(const char* path, int mode, ngmlr_b200_ctx* ctx
     counters[2] = c.host_bytes;
   }
   if (inflate_ms) *inflate_ms = c.inflate_ms;
+  if (gzip) {
+    gzip[0] = c.gzip_bytes;
+    gzip[1] = c.gzip_chunks;
+    gzip[2] = c.gzip_redecoded;
+    gzip[3] = (int64_t)(c.gzip_ms * 1000);
+  }
   close_stream(f);
   return 0;
+}
+
+
+int ngmlr_b200_debug_stream_read(const char* path, int mode, ngmlr_b200_ctx* ctx, int64_t read_size, uint8_t* out,
+                                 int64_t cap, int64_t* n_out, int32_t* error, int32_t* truncated, int64_t* counters,
+                                 float* inflate_ms) {
+  return debug_stream(path, mode, ctx, read_size, 0, out, cap, n_out, error, truncated, counters, inflate_ms, nullptr);
+}
+
+// Test hook: ngmlr_b200_debug_stream_read in mode 2 with plain gzip chunks of gzip_chunk compressed bytes (0: the
+// default or NGMLR_B200_DEBUG_GZIP_CHUNK), and gzip = {bytes the plain gzip path returned, chunks placed, chunks
+// decoded again, kernel microseconds}.
+int ngmlr_b200_debug_gzip_stream_read(const char* path, ngmlr_b200_ctx* ctx, int64_t read_size, int64_t gzip_chunk,
+                                      uint8_t* out, int64_t cap, int64_t* n_out, int32_t* error, int32_t* truncated,
+                                      int64_t* counters, int64_t* gzip) {
+  return debug_stream(path, 2, ctx, read_size, gzip_chunk, out, cap, n_out, error, truncated, counters, nullptr, gzip);
 }
 
 // Test hook: the resident read set as the device holds it -- read offsets (n_reads + 1), read lengths, the sub-read

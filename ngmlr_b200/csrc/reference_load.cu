@@ -270,6 +270,22 @@ int ngmlr_b200_load_reference_inflate_stats(ngmlr_b200_ctx* ctx, int64_t* compre
   return 0;
 }
 
+// What the plain gzip path did in the context's last load_reference (all 0 unless the FASTA file was a gzip file
+// whose first member is not BGZF, inflated on the device): bytes it returned, chunks placed, chunks decoded again
+// after a chain mismatch, kernel milliseconds. Any pointer may be NULL.
+int ngmlr_b200_load_reference_gzip_stats(ngmlr_b200_ctx* ctx, int64_t* device_bytes, int64_t* chunks,
+                                         int64_t* redecoded, float* kernel_ms) {
+  if (!ctx) return -1;
+  CsState* cs = cs_state(ctx, false);
+  if (!cs) return ctx->fail("load_reference_gzip_stats: no load");
+  const StreamCounters& c = cs->load_inflate;
+  if (device_bytes) *device_bytes = c.gzip_bytes;
+  if (chunks) *chunks = c.gzip_chunks;
+  if (redecoded) *redecoded = c.gzip_redecoded;
+  if (kernel_ms) *kernel_ms = c.gzip_ms;
+  return 0;
+}
+
 // Test hook, no context: the records read_fasta yields (host memory, not page-locked). Counts always; names (their
 // name_lens concatenated), record lengths and the concatenated sequence text where the pointers are not NULL.
 // Returns 0, or < 0 with the message in err.

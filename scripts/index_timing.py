@@ -6,8 +6,8 @@ genome (--cpu-mbp) that the CPU build finishes in reasonable time.
 
     python scripts/index_timing.py [--gbp 3] [--contigs 24] [--cpu-mbp 50] [--compressed] [--out DIR]
 
---compressed also loads the same genome as BGZF (inflated on the device) and as multi-member gzip (gzread on one host
-thread), both level 6 and written by a process pool, with their read phase and inflate counters.
+--compressed also loads the same genome as BGZF, as multi-member gzip (both written by a process pool) and as
+single-member gzip (`gzip -6`), all level 6 and inflated on the device, with their read phase and inflate counters.
 
 Phase times are host clocks around work that ends in a device synchronise (ngmlr_b200_load_reference_ms); the device
 index build alone is also timed with CUDA events (ngmlr_b200_cs_last_build_ms)."""
@@ -88,7 +88,9 @@ def load(path, gpu):
         th.join()
     return {"contigs": len(ref.names), "positions": ref.concat_len, "phases_ms": ref.ms, "wall_ms_with_context": wall,
             "inflate": {"compressed_bytes_read": ref.compressed_bytes, "device_members": ref.device_members,
-                        "host_inflated_bytes": ref.host_bytes, "inflate_kernel_ms": ref.inflate_ms},
+                        "host_inflated_bytes": ref.host_bytes, "inflate_kernel_ms": ref.inflate_ms,
+                        "gzip_device_bytes": ref.gzip_bytes, "gzip_chunks": ref.gzip_chunks,
+                        "gzip_redecoded": ref.gzip_redecoded, "gzip_kernel_ms": ref.gzip_ms},
             "index_build_kernel_ms_cuda_events": build_ms,
             "files": {"reference_written": ref.reference_written, "index_written": ref.index_written},
             "device_mem_in_use_before_GB": (total - free0) / 1e9, "device_mem_in_use_peak_GB": peak[0] / 1e9,
@@ -124,10 +126,15 @@ def main():
         if a.compressed:
             sys.path.insert(0, os.path.join(ROOT, "tests"))
             import bgzf_cases as B
-            for name, blocked in (("bgzf", True), ("gzip", False)):
+            for name, blocked in (("bgzf", True), ("gzip", False), ("gzip_single", None)):
                 path = os.path.join(work, "genome_" + name + ".fa.gz")
                 t0 = time.perf_counter()
-                size = B.compress_file(big, path, 6, blocked)
+                if blocked is None:  # one member, as `gzip -6` writes it
+                    with open(big, "rb") as src, open(path, "wb") as dst:
+                        subprocess.run(["gzip", "-6", "-c"], stdin=src, stdout=dst, check=True)
+                    size = os.path.getsize(path)
+                else:
+                    size = B.compress_file(big, path, 6, blocked)
                 out[name + "_compress_s"] = time.perf_counter() - t0
                 out[name + "_bytes"] = size
                 out[name + "_device_load"] = load(path, a.gpu)

@@ -1,10 +1,10 @@
 """Read loading speed: ngmlr_b200_reads_load (B200Aligner.load_reads) on a synthetic FASTQ shaped like bench.py's
 pacbio50 reads (lognormal lengths, median 8 000, at most 40 000 bases; 4-line records, Phred+33 qualities), plain,
-gzip and BGZF (level 6, compressed by a process pool; inflated on the device), next to the unmodified ReadProvider on
+single-member gzip (levels 1 and 6) and BGZF (level 6, compressed by a process pool), all inflated on the device, next to the unmodified ReadProvider on
 one thread (ref_read_file of oracle/_ref/libngmlr_reads.so, where built).
 
 Reports GB/s of stream text and Gbp/s of bases for each, the host read / inflate, device parse and gather phases, the
-device inflate kernel's own GB/s of output (CUDA events), and the peak device memory of the run (cudaMemGetInfo sampled
+device inflate kernels' own GB/s of output and the plain gzip path's counters (CUDA events), and the peak device memory of the run (cudaMemGetInfo sampled
 after every batch, less the level before the first load). Prints one JSON object, and writes it to --out where given.
 
     python scripts/read_load_timing.py --gb 4 [--gzip-gb 1] [--bgzf-gb 4] [--oracle-gb 0.5]"""
@@ -92,11 +92,16 @@ def time_native(path, chunk_bytes, max_bases):
                                    C.byref(dev))
     cb, dm, hb, ims = C.c_int64(0), C.c_int64(0), C.c_int64(0), C.c_float(0)
     lib.ngmlr_b200_read_file_inflate_stats(f, C.byref(cb), C.byref(dm), C.byref(hb), C.byref(ims))
+    gb, gc, gr, gms = C.c_int64(0), C.c_int64(0), C.c_int64(0), C.c_float(0)
+    lib.ngmlr_b200_read_file_gzip_stats(f, C.byref(gb), C.byref(gc), C.byref(gr), C.byref(gms))
     lib.ngmlr_b200_read_file_close(f)
     a.close()
     res = dict(seconds=dt, reads=total, gb_per_s=sb.value / dt / 1e9, read_ms=ms[0].value, parse_ms=ms[1].value,
                gather_ms=ms[2].value, handle_device_bytes=dev.value, compressed_bytes_read=cb.value,
-               device_members=dm.value, host_inflated_bytes=hb.value, inflate_kernel_ms=ims.value)
+               device_members=dm.value, host_inflated_bytes=hb.value, inflate_kernel_ms=ims.value,
+               gzip_device_bytes=gb.value, gzip_chunks=gc.value, gzip_redecoded=gr.value, gzip_kernel_ms=gms.value)
+    if gms.value > 0:
+        res["gzip_kernel_gb_per_s"] = sb.value / gms.value / 1e6
     if ims.value > 0:
         res["inflate_kernel_gb_per_s"] = sb.value / ims.value / 1e6
         res["inflate_kernel_share_of_load"] = ims.value / (dt * 1e3)
@@ -154,12 +159,15 @@ def main():
         res["bgzf"] = time_loader(bz, sb, bases, chunk, args.max_bases)
         os.unlink(bz)
     os.unlink(plain)
-    gz = os.path.join(d, "reads.fq.gz")
-    gsb, gbases, _ = write_fastq(gz, args.gzip_gb, seed=2, opener=lambda p, m: gzip.open(p, m, compresslevel=1))
-    res["gzip"] = time_loader(gz, gsb, gbases, chunk, args.max_bases)
-    res["gzip_native"] = time_native(gz, chunk, args.max_bases)
-    res["gzip"]["compressed_bytes"] = os.path.getsize(gz)
-    os.unlink(gz)
+    # single-member gzip at levels 1 and 6 (inflated on the device); "gzip" keeps its name for level 1
+    for key, level in (("gzip", 1), ("gzip6", 6)):
+        gz = os.path.join(d, "reads.fq.gz")
+        gsb, gbases, _ = write_fastq(gz, args.gzip_gb, seed=2,
+                                     opener=lambda p, m, lv=level: gzip.open(p, m, compresslevel=lv))
+        res[key] = time_loader(gz, gsb, gbases, chunk, args.max_bases)
+        res[key + "_native"] = time_native(gz, chunk, args.max_bases)
+        res[key]["compressed_bytes"] = os.path.getsize(gz)
+        os.unlink(gz)
     if args.oracle_gb > 0:
         small = os.path.join(d, "small.fq")
         osb, obases, _ = write_fastq(small, args.oracle_gb, seed=3)
