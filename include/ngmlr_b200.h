@@ -425,9 +425,8 @@ int ngmlr_b200_load_reference(ngmlr_b200_ctx* ctx, const char* fasta_path, const
 int ngmlr_b200_reference_contigs(ngmlr_b200_ctx* ctx, const char** names, int32_t* name_lens, uint64_t* starts,
                                  uint64_t* lens);
 /* What reading the FASTA file of the context's last load_reference took from the file: bytes read from it, BGZF
- * members inflated on the device, bytes inflated by the host continuation (see ngmlr_b200_read_file_inflate_stats)
- * and device inflate milliseconds; all 0 when the caches were read, gzread counts only the bytes read. Any pointer
- * may be NULL. Returns 0 or < 0. */
+ * members inflated on the device, bytes returned by the host continuation (see ngmlr_b200_read_file_inflate_stats)
+ * and device inflate milliseconds; all 0 when the caches were read. Any pointer may be NULL. Returns 0 or < 0. */
 int ngmlr_b200_load_reference_inflate_stats(ngmlr_b200_ctx* ctx, int64_t* compressed_bytes, int64_t* device_members,
                                             int64_t* host_bytes, float* inflate_ms);
 /* What the plain gzip path did in the last load_reference (see ngmlr_b200_read_file_gzip_stats); all 0 unless the
@@ -597,8 +596,10 @@ const char* ngmlr_b200_reads_load_dropped(const ngmlr_b200_read_file* f);
 int ngmlr_b200_read_file_stats(const ngmlr_b200_read_file* f, int64_t* stream_bytes, int64_t* records, float* read_ms,
                                float* parse_ms, float* gather_ms, int64_t* device_bytes);
 /* How the handle's file was inflated so far: bytes read from the file, BGZF members inflated on the device, bytes
- * inflated by the host continuation (zlib, from the first member the device could not vouch for), and milliseconds
- * of the device inflate kernel (CUDA events). Any pointer may be NULL. */
+ * returned by the host continuation (zlib's gzread reproduced on the calling thread: the whole stream of a file that
+ * is neither BGZF nor plain gzip inflated on the device, else the rest of the stream from the first member the device
+ * could not vouch for), and milliseconds of the device inflate kernel (CUDA events). So every byte of a plain text
+ * file counts in both byte counts. Any pointer may be NULL. */
 int ngmlr_b200_read_file_inflate_stats(const ngmlr_b200_read_file* f, int64_t* compressed_bytes,
                                        int64_t* device_members, int64_t* host_bytes, float* inflate_ms);
 /* What the plain gzip path (any gzip file whose first member is not BGZF) did for the handle so far: bytes it

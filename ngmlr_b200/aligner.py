@@ -37,7 +37,7 @@ class LoadedReference:
     index_written: bool
     ms: dict
     # the FASTA file's inflate (0 when the caches were read): bytes read from the file, BGZF members inflated on the
-    # device, bytes inflated by the host continuation, device inflate milliseconds
+    # device, bytes returned by the host continuation, device inflate milliseconds
     compressed_bytes: int = 0
     device_members: int = 0
     host_bytes: int = 0
@@ -226,7 +226,7 @@ class IntervalBatch:
 class ReadBatch:
     """One ngmlr_b200_reads_load call: samtext.Read records, the number of sub-reads of the resident set, and the name
     of a read ngmlr would have dropped (quality length differs from the sequence length; it ends the file). The inflate
-    counters are the handle's so far: bytes read from the file, BGZF members inflated on the device, bytes inflated by
+    counters are the handle's so far: bytes read from the file, BGZF members inflated on the device, bytes returned by
     the host continuation, device inflate milliseconds. So are the chunk counters: records resolved, the most device
     memory the handle held, chunks resolved, chunks cut short at a full line table, chunk doublings and the chunk
     capacity in bytes now. So are the plain gzip counters: bytes returned from the device, chunks placed, chunks

@@ -1,5 +1,5 @@
 // ngmlr_b200/csrc/gzip_inflate.cu -- plain gzip streams inflated on the device in rounds (the stream layer of
-// fasta.cpp drives them; the decoder core is inflate_core.cuh, shared with the BGZF kernel).
+// stream.cpp drives them; the decoder core is inflate_core.cuh, shared with the BGZF kernel).
 //
 // A gzip member is one deflate stream whose block boundaries are recorded nowhere, and a back-reference reaches up
 // to 32 KiB into output that precedes it. A round covers a span of compressed bytes that starts at a boundary known
@@ -10,7 +10,7 @@
 //      cheaply; the warp checks each survivor fully.
 //   2. k_gz_decode<false> (pass A) decodes each chunk from its start up to the first boundary at or past its stop
 //      (the next chunk's start), counting output, recording member headers / trailers and how far back the chunk's
-//      references reach before its own output. The host confirms the chain (fasta.cpp) and places the chunks.
+//      references reach before its own output. The host confirms the chain (stream.cpp) and places the chunks.
 //   3. k_gz_decode<true> (pass B) writes 16-bit symbols: a back-reference before the chunk's own output becomes the
 //      marker 256 + index into the 32 KiB window before the chunk.
 //   4. k_gz_window: one CTA walks the placed chunks in order and resolves the markers of each chunk's last 32 KiB.
@@ -20,7 +20,7 @@
 // new member (its references may not reach before its first byte).
 #include <cstdint>
 
-#include "fasta.h"
+#include "inflate.h"
 #include "inflate_core.cuh"
 
 namespace nb {

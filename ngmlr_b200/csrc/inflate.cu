@@ -1,4 +1,4 @@
-// ngmlr_b200/csrc/inflate.cu -- BGZF members inflated on the device (the stream layer of fasta.cpp launches it).
+// ngmlr_b200/csrc/inflate.cu -- BGZF members inflated on the device (the stream layer of stream.cpp launches it).
 //
 // One warp per member. Every lane runs the same bit reader and Huffman decode (shared-memory table reads broadcast),
 // so control flow stays uniform; the warp splits what is parallel: table construction (ballots / match_any over 32
@@ -16,7 +16,7 @@
 // trailer's. The host then hands the member to zlib.
 #include <cstdint>
 
-#include "fasta.h"
+#include "inflate.h"
 #include "inflate_core.cuh"
 
 namespace nb {

@@ -7,7 +7,7 @@
 #pragma once
 #include <cstdint>
 
-#include "fasta.h"  // the status codes
+#include "inflate.h"  // the status codes
 
 namespace nb {
 namespace {

@@ -2,7 +2,7 @@
 //
 // ngmlr reads its query file with ReadProvider::NextRead -> FastXParser -> kseq_read -> IParser::copyToRead
 // (src/ReadProvider.cpp:136-187, src/IParser.h:51-117, src/kseq.h:171-211) on one thread under GetNextReadBatch's
-// mutex. Here a chunk of the byte stream (plain, or inflated on the device or by zlib on the host: fasta.cpp) goes to
+// mutex. Here a chunk of the byte stream (plain, or inflated on the device or by zlib on the host: stream.cpp) goes to
 // the device once and:
 //   1. line table: one warp per 2 KiB segment counts '\n' with ballots; a scan gives every newline its rank and a
 //      second pass writes the positions. The same pass notes each segment's first '>' / '@' byte.
@@ -30,8 +30,10 @@
 #include <cub/cub.cuh>
 #include <zlib.h>
 
-#include "fasta.h"
+#include <memory>
+
 #include "runtime.h"
+#include "stream.h"
 
 using namespace nb;
 
@@ -885,11 +887,12 @@ int ngmlr_b200_reads_load(ngmlr_b200_ctx* ctx, ngmlr_b200_read_file* f, int max_
 extern "C" {
 
 // Test hook: the byte stream of a file as read_stream returns it in calls of read_size bytes, up to the first call
-// that returns less (or -1), under mode 0 = gzread, 1 = the stream layer without a device, 2 = the stream layer on
-// ctx's device and stream. Up to cap bytes are copied to out; *n_out = all bytes returned, *error = 1 when a call
-// returned -1, *truncated = stream_truncated afterwards, counters = {compressed bytes, device members, host
-// continuation bytes}, *inflate_ms the device kernel time. Returns 0, or < 0 when the file cannot be opened / bad
-// arguments / a CUDA error (message in ngmlr_b200_last_error(NULL)).
+// that returns less (or -1), under mode 0 = zlib's gzread (the oracle: gzopen, gzbuffer(1 MiB), gzread in pieces of
+// at most 1 GiB), 1 = the stream layer without a device, 2 = the stream layer on ctx's device and stream. Up to cap
+// bytes are copied to out; *n_out = all bytes returned, *error = 1 when a call returned -1, *truncated = whether the
+// stream stopped before its end (gzerror in mode 0), counters = {compressed bytes (gzoffset in mode 0), device
+// members, host continuation bytes}, *inflate_ms the device kernel time. Returns 0, or < 0 when the file cannot be
+// opened / bad arguments / a CUDA error (message in ngmlr_b200_last_error(NULL)).
 static int debug_stream(const char* path, int mode, ngmlr_b200_ctx* ctx, int64_t read_size, int64_t gzip_chunk,
                         uint8_t* out, int64_t cap, int64_t* n_out, int32_t* error, int32_t* truncated,
                         int64_t* counters, float* inflate_ms, int64_t* gzip) {
@@ -897,39 +900,67 @@ static int debug_stream(const char* path, int mode, ngmlr_b200_ctx* ctx, int64_t
     set_error_without_context("debug_stream_read: bad arguments");
     return -1;
   }
-  StreamFile* f = open_stream(path, mode == 0);
-  if (!f) {
+  gzFile gz = nullptr;
+  StreamFile* f = nullptr;
+  if (mode == 0) {
+    if ((gz = gzopen(path, "rb"))) gzbuffer(gz, 1 << 20);
+  } else {
+    f = open_stream(path);
+  }
+  if (!gz && !f) {
     set_error_without_context(std::string("debug_stream_read: cannot open ") + path);
     return -2;
   }
-  if (mode == 2 && (cudaSetDevice(ctx->device) != cudaSuccess || !bind_stream_device(f, ctx->device, ctx->stream, 0))) {
-    set_error_without_context("debug_stream_read: " + stream_error(f));
+  auto fail = [&](const std::string& e) {
+    set_error_without_context("debug_stream_read: " + e);
     close_stream(f);
     return -3;
-  }
+  };
+  if (mode == 2 && (cudaSetDevice(ctx->device) != cudaSuccess || !bind_stream_device(f, ctx->device, ctx->stream, 0)))
+    return fail(stream_error(f));
   if (mode == 2 && gzip_chunk > 0) set_gzip_chunk(f, gzip_chunk);
-  std::vector<uint8_t> buf((size_t)read_size);
+  auto read_gz = [&](uint8_t* buf, size_t n) -> int64_t {
+    size_t got = 0;
+    while (got < n) {
+      const unsigned want = (unsigned)std::min<size_t>(n - got, 1u << 30);
+      const int r = gzread(gz, buf + got, want);
+      if (r < 0) return -1;
+      got += (size_t)r;
+      if ((unsigned)r < want) break;
+    }
+    return (int64_t)got;
+  };
+  // not zero-filled: only the bytes read are touched, so read sizes of several GiB stay cheap
+  std::unique_ptr<uint8_t[]> buf(new uint8_t[(size_t)read_size]);
   int64_t total = 0;
   int32_t err = 0;
   for (;;) {
-    const int64_t r = read_stream(f, buf.data(), (size_t)read_size);
+    const int64_t r = gz ? read_gz(buf.get(), (size_t)read_size) : read_stream(f, buf.get(), (size_t)read_size);
     if (r < 0) {
       err = 1;
-      if (!stream_error(f).empty()) {
-        set_error_without_context("debug_stream_read: " + stream_error(f));
-        close_stream(f);
-        return -3;
-      }
+      if (f && !stream_error(f).empty()) return fail(stream_error(f));
       break;
     }
-    if (out && total < cap) memcpy(out + total, buf.data(), (size_t)std::min(r, cap - total));
+    if (out && total < cap) memcpy(out + total, buf.get(), (size_t)std::min(r, cap - total));
     total += r;
     if (r < read_size) break;
   }
-  const StreamCounters c = stream_counters(f);
+  StreamCounters c;
+  int32_t trunc = 0;
+  if (gz) {
+    int errnum = Z_OK;
+    gzerror(gz, &errnum);
+    trunc = errnum != Z_OK;
+    c.compressed_bytes = (int64_t)gzoffset(gz);
+    gzclose(gz);
+  } else {
+    c = stream_counters(f);
+    trunc = stream_truncated(f);
+    close_stream(f);
+  }
   if (n_out) *n_out = total;
   if (error) *error = err;
-  if (truncated) *truncated = stream_truncated(f);
+  if (truncated) *truncated = trunc;
   if (counters) {
     counters[0] = c.compressed_bytes;
     counters[1] = c.device_members;
@@ -942,10 +973,8 @@ static int debug_stream(const char* path, int mode, ngmlr_b200_ctx* ctx, int64_t
     gzip[2] = c.gzip_redecoded;
     gzip[3] = (int64_t)(c.gzip_ms * 1000);
   }
-  close_stream(f);
   return 0;
 }
-
 
 int ngmlr_b200_debug_stream_read(const char* path, int mode, ngmlr_b200_ctx* ctx, int64_t read_size, uint8_t* out,
                                  int64_t cap, int64_t* n_out, int32_t* error, int32_t* truncated, int64_t* counters,

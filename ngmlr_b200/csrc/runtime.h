@@ -20,8 +20,8 @@
 #include "../../include/ngmlr_b200.h"
 #include "cigar_text.h"
 #include "device_types.h"
-#include "fasta.h"
 #include "kernels.h"
+#include "stream.h"
 
 namespace nb {
 

@@ -11,7 +11,7 @@ import zlib
 import bgzf_cases as B
 
 MiB = 1 << 20
-# fasta.cpp: the compression ratios and the round size at which a stream stays on the device
+# stream.cpp: the compression ratios and the round size at which a stream stays on the device
 GZ_RATIO_LO, GZ_RATIO_HI, GZ_DEVICE_ROUND = 1.5, 6.5, 256 * MiB
 
 

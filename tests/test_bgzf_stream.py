@@ -1,4 +1,4 @@
-"""The BGZF stream layer on the CPU (csrc/fasta.cpp without a device binding):
+"""The BGZF stream layer on the CPU (csrc/stream.cpp without a device binding):
   - the fixtures of bgzf_cases are valid gzip, and together they reach stored, fixed and dynamic blocks, a 15-bit
     code, length 258, distance 32 768, distance-1 runs (Z_RLE), Z_HUFFMAN_ONLY and several blocks in one member;
   - the walker (members inflated with zlib's raw inflate on the host, the gzread continuation from the first member it
@@ -79,6 +79,10 @@ def test_walker_without_device_equals_gzread(files, size):
     # where the walker hands over: everything after the plain gzip member, and after the FNAME member
     for name in ("plain_gzip_after", "fname_middle", "bsize_long"):
         assert B.stream_read(lib, files[name], B.HOST, 65536)[3][2] > 0, name
+    # a file that is not BGZF: the host continuation returns every byte, and every byte of the file is read
+    text = files["plain_text"]
+    got = B.stream_read(lib, text, B.HOST, _size(text, size))
+    assert got[3] == (os.path.getsize(text), 0, len(got[0])) and len(got[0]) == os.path.getsize(text), got[3]
 
 
 def _through_pipe(tmp_path, path, mode, size):

@@ -1,4 +1,4 @@
-"""BGZF inflated on the device (csrc/inflate.cu through the stream layer of csrc/fasta.cpp):
+"""BGZF inflated on the device (csrc/inflate.cu through the stream layer of csrc/stream.cpp):
   - byte stream: the device walker returns gzread's bytes, error and truncation flag on every fixture of bgzf_cases;
   - counters: on clean files every member was inflated on the device (no host continuation), on a file with a bad
     member the device stops exactly at that member;

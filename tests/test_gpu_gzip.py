@@ -1,5 +1,5 @@
 """Plain gzip (one deflate stream per member) inflated on the device (csrc/gzip_inflate.cu through the stream layer
-of csrc/fasta.cpp), with zlib's gzread (mode 0 of the stream hook) as the oracle:
+of csrc/stream.cpp), with zlib's gzread (mode 0 of the stream hook) as the oracle:
   - clean streams give gzread's bytes and flags at read sizes 4 KiB, 65 535, 3 MiB and the whole file, at 32 KiB
     (the default) and 4 KiB chunks given explicitly, which keep a stream on the device: every byte from the device;
   - path choice: without a chunk size, a stream read in rounds too small for the device, or whose first round
