@@ -548,7 +548,7 @@ int ngmlr_b200_map_short_reads(ngmlr_b200_ctx* ctx, int read_part_length, float 
                                int64_t* first_aln, int32_t* mapped, const ngmlr_b200_sam_aln** alns,
                                int64_t* n_alns_total);
 
-/* ---- reads from a FASTA / FASTQ file (plain, gzip or BGZF): ReadProvider::NextRead -> FastXParser -> kseq_read ->
+/* ---- reads from a FASTA / FASTQ or BAM file (plain, gzip or BGZF): ReadProvider::NextRead -> FastXParser -> kseq_read ->
  * IParser::copyToRead (src/ReadProvider.cpp:136-187, src/IParser.h:51-117), parsed on the device ------------------
  * The file is read in chunks of chunk_bytes (0: 256 MiB) into page-locked memory; a chunk too small for one record
  * grows. Compressed input: a BGZF file (first member header 1f 8b 08, FLG 0x04 with a BC extra subfield, as bgzip /
@@ -567,6 +567,22 @@ int ngmlr_b200_map_short_reads(ngmlr_b200_ctx* ctx, int read_part_length, float 
  * BGZF input (which adds the compressed staging and the inflated output of a round) below 11 x max(capacity, 1 MiB),
  * and for other gzip input (which adds the compressed span, 16-bit speculative and byte output of a round, per-chunk
  * tables and the 32 KiB window) below 13 x max(capacity, 1 MiB) + 48 MiB.
+ * BAM input (no reference counterpart: ngmlr refuses BAM): a stream whose first four bytes, after any inflate, are
+ * "BAM\1" is read as BAM. A file whose inflated stream starts so is the one input read differently from ngmlr,
+ * which would parse it as FASTA / FASTQ garbage. BGZF (the usual BAM), other gzip and an uncompressed stream all work.
+ * The reads are exactly those ReadProvider makes from the text `samtools fastq -n` writes for the file: records
+ * flagged 0x100 or 0x800 are skipped (they count towards neither max_reads nor max_bases); the name is read_name cut
+ * at the first space or '\t' .. '\r', then to 249 characters; the bases are seq through "=ACMGRSVTWYHKDBN" with
+ * everything but A / C / G / T as N, reverse-complemented back under flag 0x10; the qualities are qual + 33, reversed
+ * under 0x10, and "*" when the first quality byte is 0xFF; l_seq = 0 gives an empty read. The header (text and
+ * reference entries) streams past on the host, whatever its size, without growing the chunk; nothing of it reaches
+ * the SAM. Each chunk's records are walked on the host; a record larger than the chunk doubles it. Errors, each
+ * naming the stream offset: a header or record cut off by the end of the stream, l_text / n_ref / l_name < 0,
+ * block_size < 32, fixed fields (32 + l_read_name + 4 n_cigar_op + (l_seq + 1) / 2 + l_seq) longer than block_size,
+ * l_read_name = 0 or a name without its NUL, l_seq < 0, a quality value above 93 (other than the 0xFF marker). A
+ * missing BGZF EOF block is not an error. Device memory of a handle reading BAM stays below 6 x max(capacity,
+ * 128 KiB) (the chunk, the batch's item table and its qualities), and below 8 x max(capacity, 1 MiB) for BGZF and
+ * 10 x max(capacity, 1 MiB) + 48 MiB for other gzip, with the capacity as it has grown.
  * No reference counterpart for the handle itself. */
 typedef struct ngmlr_b200_read_file ngmlr_b200_read_file;
 typedef struct {
@@ -607,6 +623,18 @@ int ngmlr_b200_read_file_inflate_stats(const ngmlr_b200_read_file* f, int64_t* c
  * time, never bytes) and kernel milliseconds. Any pointer may be NULL. */
 int ngmlr_b200_read_file_gzip_stats(const ngmlr_b200_read_file* f, int64_t* device_bytes, int64_t* chunks,
                                     int64_t* redecoded, float* kernel_ms);
+/* The format of the handle's file, decided at its first ngmlr_b200_reads_load: NGMLR_B200_READ_FORMAT_FASTX or
+ * NGMLR_B200_READ_FORMAT_BAM; -1 before. */
+#define NGMLR_B200_READ_FORMAT_FASTX 0
+#define NGMLR_B200_READ_FORMAT_BAM 1
+int ngmlr_b200_read_file_format(const ngmlr_b200_read_file* f);
+/* BAM input so far (all 0 for FASTA / FASTQ): header bytes consumed, records walked (whole records of the chunks read
+ * so far), of them skipped (flag 0x100 / 0x800), and of the others those reverse-complemented back (flag 0x10) and
+ * those without qualities (l_seq > 0, first quality byte 0xFF). For BAM, read_file_stats' records counts the records
+ * not skipped, its parse_ms is the host header and record walk and its gather_ms the chunk's upload, the decode
+ * kernels and the copy back. Any pointer may be NULL. */
+int ngmlr_b200_read_file_bam_stats(const ngmlr_b200_read_file* f, int64_t* header_bytes, int64_t* records,
+                                   int64_t* skipped, int64_t* reversed, int64_t* no_quality);
 /* Test hook: how the handle's chunks went so far -- chunks resolved, chunks cut short at a full line table, chunk
  * doublings, and the chunk capacity in bytes now. Any pointer may be NULL. */
 int ngmlr_b200_debug_read_file_chunks(const ngmlr_b200_read_file* f, int64_t* chunks, int64_t* line_limited,

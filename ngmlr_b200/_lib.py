@@ -72,8 +72,11 @@ C_API_SYMBOLS = (
     "ngmlr_b200_read_file_open", "ngmlr_b200_read_file_close", "ngmlr_b200_reads_load", "ngmlr_b200_reads_load_dropped",
     "ngmlr_b200_read_file_stats", "ngmlr_b200_read_file_inflate_stats", "ngmlr_b200_load_reference_inflate_stats",
     "ngmlr_b200_read_file_gzip_stats", "ngmlr_b200_load_reference_gzip_stats",
-    "ngmlr_b200_debug_read_file_chunks",
+    "ngmlr_b200_debug_read_file_chunks", "ngmlr_b200_read_file_format", "ngmlr_b200_read_file_bam_stats",
 )
+
+# ngmlr_b200_read_file_format (include/ngmlr_b200.h)
+READ_FORMAT_FASTX, READ_FORMAT_BAM = 0, 1
 
 # flags of ngmlr_b200_load_reference (include/ngmlr_b200.h)
 LOAD_REFERENCE_READ, LOAD_REFERENCE_WRITTEN, LOAD_INDEX_READ, LOAD_INDEX_WRITTEN = 1, 2, 4, 8
@@ -198,6 +201,8 @@ def load():
     lib.ngmlr_b200_read_file_stats.argtypes = [vp, i64p, i64p, f32p, f32p, f32p, i64p]
     lib.ngmlr_b200_read_file_inflate_stats.argtypes = [vp, i64p, i64p, i64p, f32p]
     lib.ngmlr_b200_debug_read_file_chunks.argtypes = [vp, i64p, i64p, i64p, i64p]
+    lib.ngmlr_b200_read_file_format.argtypes = [vp]
+    lib.ngmlr_b200_read_file_bam_stats.argtypes = [vp, i64p, i64p, i64p, i64p, i64p]
     lib.ngmlr_b200_load_reference_inflate_stats.argtypes = [vp, i64p, i64p, i64p, f32p]
     lib.ngmlr_b200_debug_stream_read.argtypes = [C.c_char_p, C.c_int, vp, C.c_int64, vp, C.c_int64, i64p, i32p, i32p,
                                                  i64p, f32p]

@@ -230,7 +230,9 @@ class ReadBatch:
     the host continuation, device inflate milliseconds. So are the chunk counters: records resolved, the most device
     memory the handle held, chunks resolved, chunks cut short at a full line table, chunk doublings and the chunk
     capacity in bytes now. So are the plain gzip counters: bytes returned from the device, chunks placed, chunks
-    decoded again after a chain mismatch, kernel milliseconds."""
+    decoded again after a chain mismatch, kernel milliseconds. `format` is the file's (_lib.READ_FORMAT_FASTX or
+    READ_FORMAT_BAM), and the BAM counters are the handle's so far: header bytes, records walked, of them skipped
+    (flag 0x100 / 0x800), reverse-complemented back (0x10) and without qualities."""
     reads: list
     n_sub: int
     dropped: list
@@ -248,6 +250,12 @@ class ReadBatch:
     gzip_chunks: int = 0
     gzip_redecoded: int = 0
     gzip_ms: float = 0.0
+    format: int = -1
+    bam_header_bytes: int = 0
+    bam_records: int = 0
+    bam_skipped: int = 0
+    bam_reversed: int = 0
+    bam_no_quality: int = 0
 
 
 class B200Aligner:
@@ -531,7 +539,9 @@ class B200Aligner:
         more than max_bases bases (0: no limit) -- are this context's resident read set while the batch is current,
         exactly as reads_upload would make them (cs_run / map_short_reads follow), and its `reads` are samtext.Read
         records (name, normalised bases, quality) for sam_format. A read ngmlr would drop for a quality string of
-        another length ends the file; its name is in the last batch's `dropped`."""
+        another length ends the file; its name is in the last batch's `dropped`. A BAM file (any stream that starts
+        with "BAM\\1" once inflated) gives the reads ReadProvider makes from `samtools fastq -n` of it, decoded on the
+        device."""
         from .samtext import Read, SamRead
         f = C.c_void_p()
         opts = _lib.ReadFileOptions(int(chunk_bytes))
@@ -565,8 +575,11 @@ class B200Aligner:
                     self.lib.ngmlr_b200_debug_read_file_chunks(f, *[C.byref(x) for x in ch])
                     gz = [C.c_int64(0) for _ in range(3)] + [C.c_float(0)]
                     self.lib.ngmlr_b200_read_file_gzip_stats(f, *[C.byref(x) for x in gz])
+                    bam = [C.c_int64(0) for _ in range(5)]
+                    self.lib.ngmlr_b200_read_file_bam_stats(f, *[C.byref(x) for x in bam])
                     yield ReadBatch(reads, n_sub, dropped, cb.value, dm.value, hb.value, float(ims.value), recs_n.value,
-                                    dev.value, *[x.value for x in ch], *[x.value for x in gz])
+                                    dev.value, *[x.value for x in ch], *[x.value for x in gz],
+                                    self.lib.ngmlr_b200_read_file_format(f), *[x.value for x in bam])
                 if n.value == 0:
                     break
         finally:

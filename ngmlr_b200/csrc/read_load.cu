@@ -27,11 +27,16 @@
 // length is a multiple of 16 KiB one more read returns nothing, and three things differ (all at the very end): a
 // header character that is the last byte starts an empty record with an empty name; a last line "\r" without newline
 // loses its '\r'; a quality string still ending in '\r' after the last line loses one more.
+//
+// BAM: a stream whose first four bytes (after any inflate) are "BAM\1" is read as BAM instead (bam_load.cu): the
+// header streams past on the host, the block_size chain of each chunk is walked on the host, and a batch's bases,
+// qualities and sub-read table are decoded on the device from the chunk's copy there.
 #include <cub/cub.cuh>
 #include <zlib.h>
 
 #include <memory>
 
+#include "bam.h"
 #include "runtime.h"
 #include "stream.h"
 
@@ -449,13 +454,21 @@ struct ngmlr_b200_read_file {
   int64_t records = 0, device_peak = 0;
   int64_t chunks = 0, line_limited = 0, grows = 0;  // chunks resolved, of them cut at a full line table; doublings
   float read_ms = 0, parse_ms = 0, gather_ms = 0;
+  // BAM input (format NGMLR_B200_READ_FORMAT_BAM): header, records of the chunk, the batch's items and qualities
+  int format = -1;
+  int64_t chunk_base = 0;  // stream offset of h_chunk[0]
+  BamState bam;
+  PinBuf<BamItem> h_items;
+  DevBuf<BamItem> d_items;
+  DevBuf<uint8_t> d_qual;
+  PinBuf<uint8_t> h_qual;
   size_t device_bytes() const {
     return d_chunk.owned_bytes() + d_tmp.owned_bytes() + d_fb.owned_bytes() + d_stop_flag.owned_bytes() +
            d_mark.owned_bytes() + d_seg_cnt.owned_bytes() + d_seg_mark.owned_bytes() + d_nl.owned_bytes() +
            d_sp.owned_bytes() + d_qp.owned_bytes() + d_next_pos.owned_bytes() + d_scalar.owned_bytes() +
            d_ir.owned_bytes() + d_tr.owned_bytes() + d_stops.owned_bytes() + d_mark_segs.owned_bytes() +
            d_jump.owned_bytes() + d_rec_lines.owned_bytes() + d_count.owned_bytes() + d_recs.owned_bytes() +
-           d_layout.owned_bytes() + stream_device_bytes(in);
+           d_layout.owned_bytes() + d_items.owned_bytes() + d_qual.owned_bytes() + stream_device_bytes(in);
   }
 };
 
@@ -515,6 +528,7 @@ int refill(ngmlr_b200_ctx* ctx, RF* f, bool grow) {
     }
   }
   f->h_chunk.p[f->n_host] = 0;  // a name or a quality string may end with the stream
+  f->chunk_base = f->stream_bytes - f->n_host;
   f->read_ms += (float)(now_ms() - t0);
   return 0;
 }
@@ -698,6 +712,148 @@ void assemble_quality(const RF* f, const LoadRec& r, std::string& q) {
   if ((int64_t)q.size() > r.qual_len && q.size() > 1 && q.back() == '\r') q.pop_back();
 }
 
+// BAM: the header as far as the chunk holds it, then the whole records of the chunk (host), and the chunk to the
+// device when a record is to be loaded from it.
+int bam_chunk(ngmlr_b200_ctx* ctx, RF* f) {
+  const double t0 = now_ms();
+  const uint8_t* c = f->h_chunk.p;
+  const int64_t n = f->n_host;
+  BamState& b = f->bam;
+  std::string err;
+  int64_t p = 0;
+  ++f->chunks;
+  f->n_res = n;
+  f->resolved = true;
+  f->n_good = f->next_rec = 0;
+  b.recs.clear();
+  if (!b.header_done()) {
+    const int h = bam_header(b, c, n, &p, f->chunk_base, err);
+    if (h < 0) return ctx->fail("reads_load: %s: %s", f->path.c_str(), err.c_str());
+    if (h == 0) {
+      if (f->stream_eof)
+        return ctx->fail("reads_load: %s: BAM header cut off at stream offset %lld", f->path.c_str(),
+                         (long long)(f->chunk_base + p));
+      f->tail = p;
+      f->parse_ms += (float)(now_ms() - t0);
+      return 0;
+    }
+  }
+  int64_t end = p;
+  if (bam_walk(b, c, n, p, f->chunk_base, &end, err))
+    return ctx->fail("reads_load: %s: %s", f->path.c_str(), err.c_str());
+  if (f->stream_eof && end < n)
+    return ctx->fail("reads_load: %s: BAM record cut off at stream offset %lld", f->path.c_str(),
+                     (long long)(f->chunk_base + end));
+  f->tail = end;
+  if (f->stream_eof) f->ended = true;
+  f->n_good = (int)b.recs.size();
+  int loadable = 0;
+  for (const BamRec& r : b.recs) loadable += !r.skip;
+  f->records += loadable;
+  f->parse_ms += (float)(now_ms() - t0);
+  if (loadable) {
+    const double t1 = now_ms();
+    RCU(f->d_chunk.reserve((size_t)std::max<int64_t>(f->chunk_cap, n) + 1));
+    RCU(cudaMemcpyAsync(f->d_chunk.p, c, (size_t)end, cudaMemcpyHostToDevice, ctx->stream));
+    RCU(cudaStreamSynchronize(ctx->stream));
+    f->gather_ms += (float)(now_ms() - t1);
+  }
+  return 0;
+}
+
+// BAM: the next batch of records of the chunk (skipped records pass), decoded on the device into the read arena.
+int bam_load(ngmlr_b200_ctx* ctx, RF* f, CsState* cs, int max_reads, int64_t max_bases, int read_part_length,
+             ngmlr_b200_sam_read* reads, int* n_reads) {
+  const double t0 = now_ms();
+  cudaStream_t st = ctx->stream;
+  const std::vector<BamRec>& recs = f->bam.recs;
+  std::vector<int> idx;
+  int r1 = f->next_rec;
+  int64_t bases = 0;
+  while (r1 < f->n_good && (int)idx.size() < max_reads) {
+    const BamRec& r = recs[r1];
+    if (!r.skip) {
+      if (!idx.empty() && max_bases > 0 && bases + r.l_seq > max_bases) break;
+      bases += r.l_seq;
+      idx.push_back(r1);
+    }
+    ++r1;
+  }
+  f->next_rec = r1;
+  const int n = (int)idx.size();
+  std::vector<int32_t> lens((size_t)n);
+  for (int i = 0; i < n; ++i) lens[i] = recs[idx[i]].l_seq;
+  std::vector<uint64_t> sub_start;
+  ReadSetShape shape;
+  if (read_set_layout(ctx, "reads_load", n, lens.data(), read_part_length, sub_start, shape)) return -1;
+  if (read_set_reserve(ctx, cs, n, shape)) return -1;
+  // the items: packed sequence, quality arena offset, first segment
+  CU(f->h_items.reserve((size_t)n + 1));
+  int64_t segs = 0, qbytes = 0;
+  for (int i = 0; i < n; ++i) {
+    const BamRec& r = recs[idx[i]];
+    BamItem& it = f->h_items.p[i];
+    it.seq = r.seq;
+    it.len = r.l_seq;
+    it.rev = r.rev;
+    it.seg = segs;
+    it.qual = r.qual ? qbytes : -1;
+    if (r.qual) qbytes += r.l_seq + 1;
+    segs += (r.l_seq + BAM_SEG_BASES - 1) / BAM_SEG_BASES;
+  }
+  f->h_items.p[n] = BamItem{0, -1, segs, 0, 0};
+  CU(f->h_layout.reserve(2 * ((size_t)n + 1)));
+  CU(f->d_layout.reserve(2 * ((size_t)n + 1)));
+  CU(f->d_items.reserve((size_t)n + 1));
+  CU(f->d_qual.reserve((size_t)std::max<int64_t>(qbytes, 1)));
+  CU(f->d_count.reserve(4));
+  CU(f->h_qual.reserve((size_t)std::max<int64_t>(qbytes, 1)));
+  memcpy(f->h_layout.p, ctx->read_off.data(), ((size_t)n + 1) * 8);
+  memcpy(f->h_layout.p + n + 1, sub_start.data(), ((size_t)n + 1) * 8);
+  CU(cudaMemcpyAsync(f->d_layout.p, f->h_layout.p, 2 * ((size_t)n + 1) * 8, cudaMemcpyHostToDevice, st));
+  CU(cudaMemcpyAsync(f->d_items.p, f->h_items.p, ((size_t)n + 1) * sizeof(BamItem), cudaMemcpyHostToDevice, st));
+  CU(cudaMemcpyAsync(ctx->d_read_off.p, f->d_layout.p, ((size_t)n + 1) * 8, cudaMemcpyDeviceToDevice, st));
+  CU(cudaMemsetAsync(ctx->d_reads.p, 0, shape.bytes, st));
+  if (qbytes) CU(cudaMemsetAsync(f->d_qual.p, 0, (size_t)qbytes, st));
+  CU(cudaMemsetAsync(f->d_count.p, 0x7f, 4, st));
+  bam_decode(f->d_chunk.p, f->d_items.p, n, segs, f->d_layout.p, f->d_layout.p + n + 1, read_part_length,
+             ctx->d_reads.p, f->d_qual.p, f->d_count.p, cs->d_off.p, cs->d_len.p, st);
+  CU(f->h_seq.reserve(shape.bytes + 1));
+  if (shape.bytes) CU(cudaMemcpyAsync(f->h_seq.p, ctx->d_reads.p, shape.bytes, cudaMemcpyDeviceToHost, st));
+  if (qbytes) CU(cudaMemcpyAsync(f->h_qual.p, f->d_qual.p, (size_t)qbytes, cudaMemcpyDeviceToHost, st));
+  int32_t bad = 0;
+  CU(cudaMemcpyAsync(&bad, f->d_count.p, 4, cudaMemcpyDeviceToHost, st));
+  CU(nb_stream_sync(ctx, st));
+  CU(cudaGetLastError());
+  f->device_peak = std::max<int64_t>(f->device_peak, (int64_t)f->device_bytes());
+  if (bad != 0x7f7f7f7f)
+    return ctx->fail("reads_load: %s: BAM record at stream offset %lld: a quality value above 93", f->path.c_str(),
+                     (long long)(f->chunk_base + recs[idx[bad]].name - 36));
+  read_set_install(ctx, cs, n, shape);
+  ctx->reads_h2d_bytes = (int64_t)(2 * ((size_t)n + 1) * 8 + ((size_t)n + 1) * sizeof(BamItem));
+  // the records for sam_format: names cut in place in the host chunk
+  static const char kStar[] = "*";
+  char* c = reinterpret_cast<char*>(f->h_chunk.p);
+  for (int i = 0; i < n; ++i) {
+    const BamRec& r = recs[idx[i]];
+    ngmlr_b200_sam_read& o = reads[i];
+    memset(&o, 0, sizeof(o));
+    char* name = c + r.name;
+    const int lim = std::min<int>(r.l_name - 1, NAME_CUT);
+    int k = 0;
+    while (k < lim && name[k] && !(name[k] == ' ' || (name[k] >= '\t' && name[k] <= '\r'))) ++k;
+    name[k] = 0;
+    o.name = name;
+    o.seq = reinterpret_cast<const char*>(f->h_seq.p) + ctx->read_off[i];
+    o.length = r.l_seq;
+    o.empty = r.l_seq == 0;
+    o.qual = r.qual ? reinterpret_cast<const char*>(f->h_qual.p) + f->h_items.p[i].qual : kStar;
+  }
+  f->gather_ms += (float)(now_ms() - t0);
+  *n_reads = n;
+  return (int)shape.n_sub;
+}
+
 }  // namespace
 
 extern "C" {
@@ -787,6 +943,19 @@ int ngmlr_b200_read_file_gzip_stats(const ngmlr_b200_read_file* f, int64_t* devi
   return 0;
 }
 
+int ngmlr_b200_read_file_format(const ngmlr_b200_read_file* f) { return f ? f->format : -1; }
+
+int ngmlr_b200_read_file_bam_stats(const ngmlr_b200_read_file* f, int64_t* header_bytes, int64_t* records,
+                                   int64_t* skipped, int64_t* reversed, int64_t* no_quality) {
+  if (!f) return -1;
+  if (header_bytes) *header_bytes = f->bam.header_bytes;
+  if (records) *records = f->bam.records;
+  if (skipped) *skipped = f->bam.skipped;
+  if (reversed) *reversed = f->bam.reversed;
+  if (no_quality) *no_quality = f->bam.no_quality;
+  return 0;
+}
+
 int ngmlr_b200_reads_load(ngmlr_b200_ctx* ctx, ngmlr_b200_read_file* f, int max_reads, int64_t max_bases,
                           int read_part_length, ngmlr_b200_sam_read* reads, int* n_reads, int* n_dropped) {
   if (!ctx) return -1;
@@ -807,13 +976,29 @@ int ngmlr_b200_reads_load(ngmlr_b200_ctx* ctx, ngmlr_b200_read_file* f, int max_
   CsState* cs = cs_state(ctx, true);
   f->dropped_reported = false;
   // the next chunk with a record in it
-  while (f->next_rec >= f->n_good && !f->ended) {
+  for (;;) {
+    if (f->format == NGMLR_B200_READ_FORMAT_BAM)
+      while (f->next_rec < f->n_good && f->bam.recs[f->next_rec].skip) ++f->next_rec;
+    if (f->next_rec < f->n_good || f->ended) break;
     // a record that does not fit the chunk (or its line table): a larger chunk
     const bool grow = f->resolved && f->n_good == 0 && f->tail == 0 && (f->n_host >= f->chunk_cap || f->n_res < f->n_host);
-    if (refill(ctx, f, grow) || resolve_chunk(ctx, f)) {
+    if (refill(ctx, f, grow)) {
       f->error = ctx->error;
       return -1;
     }
+    // the format, from the first bytes of the (inflated) stream
+    if (f->format < 0)
+      f->format = f->n_host >= 4 && memcmp(f->h_chunk.p, "BAM\1", 4) == 0 ? NGMLR_B200_READ_FORMAT_BAM
+                                                                          : NGMLR_B200_READ_FORMAT_FASTX;
+    if (f->format == NGMLR_B200_READ_FORMAT_BAM ? bam_chunk(ctx, f) : resolve_chunk(ctx, f)) {
+      f->error = ctx->error;
+      return -1;
+    }
+  }
+  if (f->format == NGMLR_B200_READ_FORMAT_BAM) {
+    const int r = bam_load(ctx, f, cs, max_reads, max_bases, read_part_length, reads, n_reads);
+    if (r < 0) f->error = ctx->error;
+    return r;
   }
   const double t0 = now_ms();
   int r0 = f->next_rec, r1 = r0;
