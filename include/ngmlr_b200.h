@@ -505,6 +505,42 @@ int ngmlr_b200_sam_format(const ngmlr_b200_sam_options* opts, int64_t n_reads, c
                           const ngmlr_b200_sam_aln* alns, int n_refs, const char* const* ref_names,
                           const int32_t* ref_name_lens, char* out, size_t cap, size_t* written);
 
+/* ---- BAM records of the same batches (no reference counterpart: ngmlr writes only SAM) ----------------------
+ * The records are exactly what `samtools view -b` makes of the text ngmlr_b200_sam_header / ngmlr_b200_sam_format
+ * write for the same arguments (SAMv1 section 4.2), without the BGZF framing (ngmlr_b200_bgzf_* adds it):
+ *   refID: the index of the header @SQ whose SN is the printed RNAME (-1 for "*"); next_refID / next_pos -1, tlen 0;
+ *   pos: the printed POS - 1; a POS above 2^31 is an error (htslib's bam_write1 refuses it too);
+ *   mapq and flag as printed (mapq outside 0..255 is an error); l_read_name counts the NUL (a name of more than 254
+ *   bytes is an error);
+ *   CIGAR: parsed from the text, "*" = no operations. Above 65535 operations without bam_cigar_fix: SAMv1's
+ *   placeholder <l_seq>S<rlen>N, and the real CIGAR as a CG:B:I tag appended last (as htslib writes it). With
+ *   bam_cigar_fix the text already holds <length>S and CG:B:I, which are encoded as they stand;
+ *   bin: reg2bin(pos, pos + max(rlen, 1)) with rlen from the CIGAR as encoded; 4680 for an unmapped record;
+ *   SEQ through "=ACMGRSVTWYHKDBN" (lower case as upper case, anything else as N); QUAL as char - 33, "*" as l_seq
+ *   bytes of 0xFF (the quality orientation of ngmlr_b200_sam_options applies, as it does to the text);
+ *   tags in text order: i as htslib's smallest type (c / s / i below 0, else C / S / I), f as (float)strtod of the
+ *   printed text, Z with its NUL, B:I as a count and uint32 values.
+ * Which alignments get a record, the flags, the strand of the qualities, SA:Z and the long-CIGAR case are decided by
+ * the same code for both formats. */
+
+/* The BAM header: "BAM\1", l_text and the text ngmlr_b200_sam_header writes (no NUL), n_ref, and per @SQ its name
+ * with a NUL and its LN. Returns 0 and sets *written; -2 with *written = the bytes needed when cap is too small;
+ * -1 on invalid arguments or an LN above 2^31 - 1 (ngmlr_b200_last_error(NULL) says which). */
+int ngmlr_b200_bam_header(int n_refs, const char* const* ref_names, const uint64_t* ref_lens, const char* version,
+                          const char* command_line, const ngmlr_b200_sam_options* opts,
+                          const char* const* rg_fields, char* out, size_t cap, size_t* written);
+
+/* The BAM records (block_size first) of n_reads reads in read order, sized and written by host threads as
+ * ngmlr_b200_sam_format. ref_names / ref_name_lens are sam_format's names per ref_id; the n_targets header names
+ * target_names (the ref_names of ngmlr_b200_bam_header) give refID. Returns 0 and sets *written; -2 with *written =
+ * the bytes needed when cap is too small (nothing is written then); -1 on invalid arguments or a record BAM cannot
+ * hold (POS above 2^31, an RNAME not in the header, mapq outside 0..255, a name of more than 254 bytes, a malformed
+ * CIGAR, a QUAL of another length than SEQ): ngmlr_b200_last_error(NULL) names the first such read. */
+int ngmlr_b200_bam_format(const ngmlr_b200_sam_options* opts, int64_t n_reads, const ngmlr_b200_sam_read* reads,
+                          const ngmlr_b200_sam_aln* alns, int n_refs, const char* const* ref_names,
+                          const int32_t* ref_name_lens, int n_targets, const char* const* target_names, char* out,
+                          size_t cap, size_t* written);
+
 /* ---- reads of at most read_part_length bases: ScoreBuffer::scoreShortRead + AlignmentBuffer::processShortRead --
  * ngmlr does not split such a read (src/ReadProvider.cpp:152-156); CS::SendToBuffer (src/CS.cpp:307-316) sends it to
  * scoreShortRead instead of the sub-read scorer and the chaining code. cs_run scores its candidates with the sub-read
@@ -639,6 +675,42 @@ int ngmlr_b200_read_file_bam_stats(const ngmlr_b200_read_file* f, int64_t* heade
  * doublings, and the chunk capacity in bytes now. Any pointer may be NULL. */
 int ngmlr_b200_debug_read_file_chunks(const ngmlr_b200_read_file* f, int64_t* chunks, int64_t* line_limited,
                                       int64_t* grows, int64_t* chunk_cap);
+
+/* ---- BGZF output with the deflate on the device (BAM, or BGZF-compressed SAM) ----------------------------------
+ * No reference counterpart. A handle compresses any byte stream into a BGZF file as htslib lays it out: the stream is
+ * cut into blocks of 0xff00 input bytes, and only ngmlr_b200_bgzf_flush and ngmlr_b200_bgzf_close end a block
+ * early (a BAM writer flushes after the header, as htslib does). Each member carries htslib's header bytes (1f 8b 08
+ * 04, MTIME 0, XFL 0, OS 0xff, XLEN 6, the BC subfield with BSIZE), a raw deflate stream, CRC32 and ISIZE; close
+ * appends the 28-byte EOF block. Each block is deflated on the device: matches of 4 to 258 bytes within 32 KiB
+ * (the nearest of up to 4 prior occurrences of the same 4 bytes, longest first), a greedy parse, and the smallest of
+ * a dynamic Huffman, fixed Huffman or stored block by exact bit count, so no member exceeds 65 536 bytes and an
+ * incompressible block costs 31 bytes of framing. The file depends only on the bytes written and the flush points:
+ * not on how writes are split, on chunk_bytes or on timing.
+ * The handle owns two page-locked staging buffers of chunk_bytes (0: 64 MiB; rounded down to whole blocks, at least
+ * one) and its own CUDA stream on the context's device, which does not wait for the context's streams: while one batch
+ * compresses the caller fills the other buffer, and the host writes the batch before to the file. Device memory of a
+ * handle stays below 20 x chunk_bytes + 64 MiB. Errors (the file cannot be opened, a short write, any CUDA error)
+ * return < 0 and leave the handle failed; ngmlr_b200_bgzf_last_error says what happened. There is no CPU fallback:
+ * without a device there is no context and no handle. */
+typedef struct ngmlr_b200_bgzf_writer ngmlr_b200_bgzf_writer;
+typedef struct {
+  int64_t chunk_bytes; /* page-locked staging per batch; 0 = 64 MiB; at most 1 GiB */
+} ngmlr_b200_bgzf_options;
+/* opts may be NULL. Returns 0, or < 0 (ngmlr_b200_last_error(NULL) describes it). */
+int ngmlr_b200_bgzf_open(ngmlr_b200_ctx* ctx, const char* path, const ngmlr_b200_bgzf_options* opts,
+                         ngmlr_b200_bgzf_writer** out);
+int ngmlr_b200_bgzf_write(ngmlr_b200_bgzf_writer* w, const void* buf, size_t n);
+/* Ends the current block (if it holds any byte) and waits until every byte written so far is in the file. */
+int ngmlr_b200_bgzf_flush(ngmlr_b200_bgzf_writer* w);
+/* Flushes, appends the EOF block, closes the file and frees the handle (also on failure). Returns 0, or < 0 with
+ * ngmlr_b200_last_error(NULL) describing the first error of the handle. */
+int ngmlr_b200_bgzf_close(ngmlr_b200_bgzf_writer* w);
+const char* ngmlr_b200_bgzf_last_error(const ngmlr_b200_bgzf_writer* w);
+/* Bytes written to the handle, bytes of its members in the file (the EOF block not counted), members, members
+ * written as stored blocks, milliseconds of device work (CUDA events, copies excluded), and the device memory the
+ * handle holds. Any pointer may be NULL. */
+int ngmlr_b200_bgzf_stats(const ngmlr_b200_bgzf_writer* w, int64_t* bytes_in, int64_t* bytes_out, int64_t* blocks,
+                          int64_t* stored_blocks, float* device_ms, int64_t* device_bytes);
 
 #ifdef __cplusplus
 }

@@ -73,6 +73,8 @@ C_API_SYMBOLS = (
     "ngmlr_b200_read_file_stats", "ngmlr_b200_read_file_inflate_stats", "ngmlr_b200_load_reference_inflate_stats",
     "ngmlr_b200_read_file_gzip_stats", "ngmlr_b200_load_reference_gzip_stats",
     "ngmlr_b200_debug_read_file_chunks", "ngmlr_b200_read_file_format", "ngmlr_b200_read_file_bam_stats",
+    "ngmlr_b200_bam_header", "ngmlr_b200_bam_format", "ngmlr_b200_bgzf_open", "ngmlr_b200_bgzf_write",
+    "ngmlr_b200_bgzf_flush", "ngmlr_b200_bgzf_close", "ngmlr_b200_bgzf_last_error", "ngmlr_b200_bgzf_stats",
 )
 
 # ngmlr_b200_read_file_format (include/ngmlr_b200.h)
@@ -87,6 +89,10 @@ class ReferenceOptions(C.Structure):
 
 
 class ReadFileOptions(C.Structure):
+    _fields_ = [("chunk_bytes", C.c_int64)]
+
+
+class BgzfOptions(C.Structure):
     _fields_ = [("chunk_bytes", C.c_int64)]
 
 
@@ -211,6 +217,13 @@ def load():
     lib.ngmlr_b200_debug_gzip_stream_read.argtypes = [C.c_char_p, vp, C.c_int64, C.c_int64, vp, C.c_int64, i64p, i32p,
                                                       i32p, i64p, i64p]
     lib.ngmlr_b200_debug_resident_reads.argtypes = [vp, i32p, i32p, i64p, vp, vp, vp, vp, vp]
+    lib.ngmlr_b200_bgzf_open.argtypes = [vp, C.c_char_p, C.POINTER(BgzfOptions), C.POINTER(vp)]
+    lib.ngmlr_b200_bgzf_write.argtypes = [vp, vp, C.c_size_t]
+    lib.ngmlr_b200_bgzf_flush.argtypes = [vp]
+    lib.ngmlr_b200_bgzf_close.argtypes = [vp]
+    lib.ngmlr_b200_bgzf_last_error.argtypes = [vp]
+    lib.ngmlr_b200_bgzf_last_error.restype = C.c_char_p
+    lib.ngmlr_b200_bgzf_stats.argtypes = [vp, i64p, i64p, i64p, i64p, f32p, i64p]
     lib.ngmlr_b200_sw_last_kernel_ms.argtypes = [vp]
     lib.ngmlr_b200_sw_last_kernel_ms.restype = C.c_float
     lib.ngmlr_b200_plugin_context.argtypes = [vp]

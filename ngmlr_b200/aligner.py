@@ -258,6 +258,64 @@ class ReadBatch:
     bam_no_quality: int = 0
 
 
+class BgzfWriter:
+    """A BGZF file written through a context's device (ngmlr_b200_bgzf_*): write() any bytes, flush() to end the
+    current block and put everything written so far into the file, close() to add the EOF block. Usable as a context
+    manager. stats(): bytes in, bytes of members out (the EOF block not counted), members, stored members, device
+    milliseconds, device bytes held."""
+
+    def __init__(self, lib, ctx, path, chunk_bytes=0):
+        self.lib = lib
+        self.h = C.c_void_p()
+        opts = _lib.BgzfOptions(int(chunk_bytes))
+        if lib.ngmlr_b200_bgzf_open(ctx, os.fsencode(path), C.byref(opts), C.byref(self.h)) != 0:
+            self.h = None
+            raise RuntimeError(lib.ngmlr_b200_last_error(None).decode())
+        self._final = None
+
+    def _check(self, rc):
+        if rc < 0:
+            raise RuntimeError(self.lib.ngmlr_b200_bgzf_last_error(self.h).decode())
+
+    def write(self, data):
+        data = bytes(data)
+        self._check(self.lib.ngmlr_b200_bgzf_write(self.h, data, len(data)))
+
+    def flush(self):
+        self._check(self.lib.ngmlr_b200_bgzf_flush(self.h))
+
+    def stats(self):
+        if self.h is None:
+            return self._final
+        v = [C.c_int64(0) for _ in range(4)] + [C.c_float(0), C.c_int64(0)]
+        self.lib.ngmlr_b200_bgzf_stats(self.h, *[C.byref(x) for x in v])
+        keys = ("bytes_in", "bytes_out", "blocks", "stored_blocks", "device_ms", "device_bytes")
+        return dict(zip(keys, [x.value for x in v]))
+
+    def close(self):
+        h = self.h
+        if h is None:
+            return
+        if self.lib.ngmlr_b200_bgzf_flush(h) == 0:
+            self._final = self.stats()
+        self.h = None
+        if self.lib.ngmlr_b200_bgzf_close(h) != 0:
+            raise RuntimeError(self.lib.ngmlr_b200_last_error(None).decode())
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def __del__(self):
+        # a handle dropped without close() still frees its buffers; an error it met has nobody left to report to
+        try:
+            self.close()
+        except RuntimeError:
+            pass
+
+
 class B200Aligner:
     def __init__(self, gpu_id=0, scoring=DEFAULT_SCORING, stream=None):
         self.lib = _lib.load()
@@ -584,6 +642,11 @@ class B200Aligner:
                     break
         finally:
             self.lib.ngmlr_b200_read_file_close(f)
+
+    def bgzf_writer(self, path, chunk_bytes=0):
+        """A BgzfWriter on this context's device: BAM (samtext.bam_header, then flush(), then samtext.bam_format
+        batches) or BGZF-compressed SAM. chunk_bytes: page-locked staging per batch (0: 64 MiB)."""
+        return BgzfWriter(self.lib, self.h, path, chunk_bytes)
 
     def resident_reads(self):
         """Test aid: the resident read set as the device holds it -- (read offsets, read lengths, sub-read offsets,

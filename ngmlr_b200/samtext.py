@@ -66,6 +66,14 @@ def _bind(lib):
     lib.ngmlr_b200_sam_format.argtypes = [C.POINTER(SamOptions), C.c_int64, C.POINTER(SamRead), C.POINTER(SamAln),
                                           C.c_int, C.POINTER(C.c_char_p), C.POINTER(C.c_int32), C.c_void_p,
                                           C.c_size_t, C.POINTER(C.c_size_t)]
+    lib.ngmlr_b200_bam_header.restype = C.c_int
+    lib.ngmlr_b200_bam_header.argtypes = [C.c_int, C.POINTER(C.c_char_p), C.POINTER(C.c_uint64), C.c_char_p,
+                                          C.c_char_p, C.POINTER(SamOptions), C.POINTER(C.c_char_p), C.c_void_p,
+                                          C.c_size_t, C.POINTER(C.c_size_t)]
+    lib.ngmlr_b200_bam_format.restype = C.c_int
+    lib.ngmlr_b200_bam_format.argtypes = [C.POINTER(SamOptions), C.c_int64, C.POINTER(SamRead), C.POINTER(SamAln),
+                                          C.c_int, C.POINTER(C.c_char_p), C.POINTER(C.c_int32), C.c_int,
+                                          C.POINTER(C.c_char_p), C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]
     lib._sam_bound = True
 
 
@@ -132,6 +140,73 @@ def sam_format(reads, ref_names, write_unmapped=True, bam_cigar_fix=False, fix_q
     buf = C.create_string_buffer(cap_ + 1)
     rc = lib.ngmlr_b200_sam_format(C.byref(opts), packed.n, packed.reads, packed.alns, n, names, name_lens, buf, cap_,
                                    C.byref(written))
+    if cap is not None:
+        return rc, written.value, buf.raw[:written.value] if rc == 0 else b""
+    assert rc == 0, rc
+    return buf.raw[:written.value]
+
+
+def _bam_error(lib):
+    return RuntimeError(lib.ngmlr_b200_last_error(None).decode())
+
+
+def bam_header(ref_names, ref_lens, version=b"0.2.8", command_line=b"ngmlr", rg_id=None, rg_fields=None):
+    """The BAM header whose text is sam_header's for the same arguments (ngmlr_b200_bam_header). Raises
+    RuntimeError for an LN above 2^31 - 1."""
+    lib = _lib.load()
+    _bind(lib)
+    n = len(ref_names)
+    names = (C.c_char_p * max(n, 1))(*ref_names)
+    lens = (C.c_uint64 * max(n, 1))(*ref_lens)
+    opts = _options(1, 0, 0, 1, rg_id)
+    fields = None
+    if rg_fields is not None:
+        assert len(rg_fields) == 11
+        fields = (C.c_char_p * 11)(*rg_fields)
+    need = C.c_size_t(0)
+    rc = lib.ngmlr_b200_bam_header(n, names, lens, version, command_line, C.byref(opts), fields, None, 0,
+                                   C.byref(need))
+    if rc == -1:
+        raise _bam_error(lib)
+    buf = C.create_string_buffer(need.value)
+    rc = lib.ngmlr_b200_bam_header(n, names, lens, version, command_line, C.byref(opts), fields, buf, need.value,
+                                   C.byref(need))
+    assert rc == 0, rc
+    return buf.raw[:need.value]
+
+
+def bam_format(reads, ref_names, target_names=None, write_unmapped=True, bam_cigar_fix=False,
+               fix_quality_orientation=False, threads=0, rg_id=None, cap=None):
+    """BAM records of `reads` (list of Read or a PackedReads) in read order: what samtools makes of sam_format's text
+    for the same arguments (ngmlr_b200_bam_format). target_names: the header's contig names (default: ref_names
+    without repeats, in order). Raises RuntimeError for a record BAM cannot hold. With cap: (rc, bytes needed,
+    records)."""
+    lib = _lib.load()
+    _bind(lib)
+    packed = reads if isinstance(reads, PackedReads) else PackedReads(reads)
+    if target_names is None:
+        target_names = list(dict.fromkeys(ref_names))
+    n, nt = len(ref_names), len(target_names)
+    names = (C.c_char_p * max(n, 1))(*ref_names)
+    name_lens = (C.c_int32 * max(n, 1))(*[len(x) for x in ref_names])
+    targets = (C.c_char_p * max(nt, 1))(*target_names)
+    opts = _options(write_unmapped, bam_cigar_fix, fix_quality_orientation, threads, rg_id)
+    written = C.c_size_t(0)
+
+    def call(buf, size):
+        rc = lib.ngmlr_b200_bam_format(C.byref(opts), packed.n, packed.reads, packed.alns, n, names, name_lens, nt,
+                                       targets, buf, size, C.byref(written))
+        if rc == -1:
+            raise _bam_error(lib)
+        return rc
+
+    if cap is None:
+        call(None, 0)
+        cap_ = written.value
+    else:
+        cap_ = cap
+    buf = C.create_string_buffer(cap_ + 1)
+    rc = call(buf, cap_)
     if cap is not None:
         return rc, written.value, buf.raw[:written.value] if rc == 0 else b""
     assert rc == 0, rc
